@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""Benchmarks of the hot path on N B200s of one node, one JSON line on stdout (rank 0).
+"""Benchmarks of the hot path on N H100s of one node, one JSON line on stdout (rank 0).
 
     python bench.py --gpus N --steps K --warmup W                 # headline: BASELINE.json configs[1] (cfg2)
     python bench.py --config cfg3|cfg4|cfg4-ais|cfg5|cfg5-pcd      # the other BASELINE.json configurations
     python bench.py --impl reference [--config ...]                # the reference's CPU path (oracle restatement), host cores
+    python bench.py ... --dump-outputs DIR                          # also write what the last timed step computed, as DIR/*.npy
 
 cfg2      BernoulliRBM 784-1024, batch 4096 per GPU, CD-5               metric: Gibbs updates/s (batch x k)
 cfg3      GaussianRBM 3072-5000, batch 2048, CD-1                        metric: Gibbs updates/s
@@ -30,11 +31,10 @@ for _p in (ROOT, os.path.join(ROOT, 'boltzmann-machines_b200')):
 
 # ---- the headline workload (kept as module constants: tools/ and tests/ import them) -------------------------
 V, H, B, K_GIBBS = 784, 1024, 4096, 5
-N_BATCHES = int(os.environ.get('BM_BENCH_BATCHES', '40'))    # resident dataset: 40 x 4096 rows = 257 MB of bf16 > 126 MB L2
+N_BATCHES = int(os.environ.get('BM_BENCH_BATCHES', '40'))    # resident dataset: 40 x 4096 rows = 257 MB of bf16 > 50 MB L2
 #                                      (BM_BENCH_BATCHES: dry runs on the host simulation only -- `config.l2_policy` states the size)
 LR, MOMENTUM, L2 = 0.05, 0.5, 1e-5
 REFERENCE_BUDGET_S = float(os.environ.get('BM_BENCH_REFERENCE_SECONDS', '40'))   # --impl reference: timed + warm-up steps together
-FIT_MIN_STEPS = int(os.environ.get('BM_BENCH_FIT_STEPS', '2000'))   # e2e: fit() runs at least this many steps (50 epochs of 40 batches)
 FLOP_PER_STEP = 2.0 * B * V * H * (2 * K_GIBBS + 3)      # SURVEY.md §8(d): (2k+3) GEMMs of 2BVH
 
 RBM_WORKLOADS = {
@@ -193,23 +193,9 @@ def measured_peaks():
     if os.path.isfile(p):
         with open(p) as fh:
             d = json.load(fh)
-        burst = float(d.get('bf16_tflops', 1590.0))
+        burst = float(d.get('bf16_tflops', 989.0))
         return burst, float(d.get('bf16_tflops_sustained', burst)), 'measured (MEASURED_PEAKS.json bf16_tflops / bf16_tflops_sustained)'
-    return 1590.0, 1400.0, 'fallback (B200_PROFILING.md: 1.59 PFLOP/s burst, ~1.4 sustained)'
-
-
-def recorded_traffic(kernel_key):
-    """dram bytes per launch of the dominant kernel from the committed `ncu --set full` capture (profiles/...traffic.json states
-    the commit it was taken at); None when this configuration has no capture."""
-    p = os.path.join(ROOT, 'profiles', 'tc_program_kernel_traffic.json')
-    if os.path.isfile(p):
-        with open(p) as fh:
-            d = json.load(fh)
-        if kernel_key in d:
-            return d[kernel_key]
-        if kernel_key == 'cfg2':
-            return d.get('dram_bytes_per_launch')
-    return None
+    return 989.0, 989.0, 'H100 SXM data sheet: 989 TFLOP/s dense bf16 (700 W part); not measured'
 
 
 def blas_threads():
@@ -285,6 +271,7 @@ def rbm_workload(name, ctx, rank, world, compute):
               cfg_extra={'global_batch': b * world, 'k': k},
               kernel='bm::tc_program_kernel<2>')
     wl['step'] = lambda i: eng.train_step_at((i % n_batches) * b, b, lr, MOMENTUM, k, seed, i)
+    wl['outputs'] = lambda: eng.get_params(['W', 'vb', 'hb'])           # the model a training step leaves behind
 
     def e2e_factory(kind_of_feed):
         # 'native': what fit() feeds for this data (bytes for binary data); 'float32': the same rows as grey levels --
@@ -414,6 +401,7 @@ def dbm_workload(name, ctx, rank, world, compute, ais_runs, ais_betas):
             return {'log_Z': float(np.logaddexp.reduce(lw) - np.log(len(lw)))}
         wl['quality'] = quality
         wl['sync_each_step'] = True
+        wl['outputs'] = lambda: {'ais_log_weights': last['logw']}        # what eng.ais returns
         return wl
     sizes = [v] + hs
     pairs = sum(sizes[i] * sizes[i + 1] for i in range(len(hs)))
@@ -443,6 +431,7 @@ def dbm_workload(name, ctx, rank, world, compute, ais_runs, ais_betas):
     wl['h2d'] = b * v * 4 * world
     wl['d2h'] = 16 * world
     wl['quality'] = lambda: {key: float(val) for key, val in nmf.items()}
+    wl['outputs'] = lambda: eng.get_params()                           # the model a training step leaves behind
     return wl
 
 
@@ -512,7 +501,7 @@ METRICS = {'cfg4': ('dbm_train_rows_per_sec', 'rows/s'), 'cfg4-ais': ('ais_chain
 
 def run_reference(args):
     """The reference arm: the reference's own CPU path (oracle/ -- TF 1.3 / Python 2 cannot run in this image, DESIGN section 6) on
-    the host cores, with the BLAS pool at its fastest size.  Same `config`, `metric`, `unit` as the b200 arm; RBM workloads run
+    the host cores, with the BLAS pool at its fastest size.  Same `config`, `metric`, `unit` as the CUDA arm; RBM workloads run
     exactly --steps timed and --warmup untimed steps, each a bounded sample of the workload's step (cpu_arm)."""
     rank = int(os.environ.get('RANK', '0'))
     if rank != 0:
@@ -541,21 +530,48 @@ def run_reference(args):
 
 
 # --------------------------------------------------------------------------------------------
+DUMP_BYTES = 64 * 10 ** 6       # --dump-outputs: at most 64 MB in all
+
+
+def dump_outputs(path, arrays):
+    """Writes `arrays` ({name: array}) as path/<name>.npy in float32 (float64 stays float64).  An array that would take the total
+    past DUMP_BYTES is replaced by a fixed, seeded sample of its elements (flattened, sorted indices; `<name>_index.npy` holds
+    them), so that two builds run with the same arguments can be compared output for output."""
+    os.makedirs(path, exist_ok=True)
+    arrays = {k: np.asarray(v, dtype=np.float64 if np.asarray(v).dtype == np.float64 else np.float32) for k, v in arrays.items()}
+    left = DUMP_BYTES
+    for name in sorted(arrays, key=lambda k: arrays[k].nbytes):
+        a = arrays[name]
+        share = left // max(1, sum(1 for k in arrays if arrays[k].nbytes >= a.nbytes))
+        if a.nbytes > share:
+            n = max(1, share // (a.itemsize + 8))
+            idx = np.sort(np.random.RandomState(12345).choice(a.size, size=n, replace=False))
+            np.save(os.path.join(path, name + '_index.npy'), idx.astype(np.int64))
+            a = a.reshape(-1)[idx]
+            left -= idx.nbytes
+        np.save(os.path.join(path, name + '.npy'), a)
+        left -= a.nbytes
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
     ap.add_argument('--steps', type=int, default=None)
     ap.add_argument('--warmup', type=int, default=10)
-    ap.add_argument('--impl', default='b200')
+    ap.add_argument('--impl', default='cuda', choices=('cuda', 'reference'))
     ap.add_argument('--config', default='cfg2', choices=WORKLOAD_NAMES)
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--compute', default='bf16')
     ap.add_argument('--ais-runs', type=int, default=20000)
     ap.add_argument('--ais-betas', type=int, default=1000)
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last one computed as DIR/<name>.npy (float32 / float64)')
     args = ap.parse_args()
     if args.steps is None:
         args.steps = {'cfg2': 2000, 'cfg3': 500, 'cfg5': 300, 'cfg5-pcd': 200, 'cfg4': 300, 'cfg4-ais': 3}[args.config]
     if args.impl == 'reference':
+        if args.dump_outputs:
+            ap.error('--dump-outputs writes what the CUDA arm computed: not available with --impl reference')
         return run_reference(args)
     args.warmup = max(args.warmup, 3)
     if args.config == 'cfg4-ais':
@@ -621,6 +637,8 @@ def main():
     launches = ctx.launch_count() - l0
     ms = max_over_ranks(ms)
     value = args.steps * units * world / (ms * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, wl['outputs']())
 
     # ---- region 2: same steps with per-launch CUDA events on the tensor-core kernel ---------------------------------
     ctx.profile_tc(True)
@@ -665,10 +683,9 @@ def main():
         # the headline end-to-end number goes through the public API itself: Model(...).fit(X)
         e2e['e2e_epoch_call'] = e2e.pop('e2e')
         barrier()
-        # fit() pays one-time costs (engine construction, packing and page-locking the training set, the save: about 0.1 s for
-        # this 514 MB float32 set) that a K-step run does not amortise when K is a few dozen: the fit runs for at least
-        # FIT_MIN_STEPS steps (whole epochs) whatever K is, and states how many it ran
-        fit_target = max(args.steps, FIT_MIN_STEPS if args.config == 'cfg2' else args.steps)
+        # fit() runs whole epochs: K steps rounded up to whole epochs, and the line states how many it ran.  Its one-time
+        # costs (engine construction, packing and page-locking the training set, the save) are not amortised at small K.
+        fit_target = args.steps
         try:
             fit_s, fit_steps, up = wl['fit_e2e'](min(fit_target, 2 * wl['n_batches']), barrier)          # (warm: library loaded, CUDA context up)
             passes = []
@@ -764,7 +781,7 @@ def main():
         'roofline': {'bound': 'tensor', 'achieved': achieved, 'peak': peak, 'unit': 'TFLOP/s',
                      'frac': achieved / peak if peak else None,
                      'peak_sustained': peak_sustained, 'frac_sustained': achieved / peak_sustained if peak_sustained else None,
-                     'traffic': recorded_traffic(args.config),
+                     'traffic': None,                 # (no DRAM capture of the kernel on the H100)
                      'kernel': wl['kernel'], 'launches': int(tc_launches), 'peak_source': peak_src,
                      'achieved_is': 'algorithmic FLOPs of the tensor-core launches / their CUDA-event time (region 2)',
                      'step_tflops': step_tflops, 'step_frac': step_tflops / peak, 'step_frac_sustained': step_tflops / peak_sustained},

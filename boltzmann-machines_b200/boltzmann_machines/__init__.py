@@ -1,6 +1,6 @@
-"""B200-native RBM/DBM engine behind the yell/boltzmann-machines Python API.
+"""H100-native RBM/DBM engine behind the yell/boltzmann-machines Python API.
 
-Host side: thin Python (this package).  Compute: hand-written sm_100a CUDA in
+Host side: thin Python (this package).  Compute: hand-written sm_90a CUDA in
 ``../csrc`` reached through the C-ABI of ``include/bm.h`` (``libbm.so``).
 """
 from . import base

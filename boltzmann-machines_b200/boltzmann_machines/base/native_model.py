@@ -7,7 +7,7 @@ methods (``init``, ``fit``, ``load_model``, ``get_tf_params``,
 (``params.json`` + ``random_state.json`` next to the weights) and the same
 error behaviour (``RuntimeError`` before ``fit``/``init``), but instead of a
 ``tf.Session`` a decorated call runs against an *engine*: a handle into
-``libbm.so`` (hand-written sm_100a CUDA behind the C-ABI of ``include/bm.h``).
+``libbm.so`` (hand-written sm_90a CUDA behind the C-ABI of ``include/bm.h``).
 
 The engine is produced by a factory looked up in ``ENGINE_FACTORIES``.  The
 default factories come from ``boltzmann_machines._native`` and raise loudly when

@@ -7,7 +7,7 @@ builds a TF graph (``_make_tf_model``) this class hands a configuration to the
 engine (``_make_engine``); where it calls ``session.run(train_op, feed_dict)``
 per mini-batch (:566) this class makes one C-ABI call, ``engine.train_step``,
 which runs the whole CD-k step -- h0, k Gibbs sweeps, dW/dvb/dhb, sparsity,
-momentum update -- in hand-written sm_100a CUDA.
+momentum update -- in hand-written sm_90a CUDA.
 """
 import numpy as np
 

@@ -151,7 +151,7 @@ using namespace bm;
 
 extern "C" {
 
-const char* bm_version(void) { return "bm-b200 0.1 (sm_100a)"; }
+const char* bm_version(void) { return "bm 0.1 (sm_90a)"; }
 const char* bm_last_error(void) { return g_last_error.c_str(); }
 
 int bm_device_count(int* n) {
@@ -176,9 +176,9 @@ int bm_ctx_create(int device, bm_ctx** out) {
     BM_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     BM_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10)
+    if (prop.major != 9 || prop.minor != 0)
         throw Error(BM_ENOGPU, std::string("device is sm_") + std::to_string(prop.major) + std::to_string(prop.minor) +
-                                   "; libbm.so is built for sm_100a (B200) only");
+                                   "; libbm.so is built for sm_90a (H100) only");
     Ctx* c = new Ctx();
     c->device = device;
     c->sm_count = prop.multiProcessorCount;
@@ -240,7 +240,7 @@ int bm_ctx_flush_l2(bm_ctx* h) {
     Ctx* c = reinterpret_cast<Ctx*>(h);
     BM_REQUIRE(c, "null context");
     if (!c->l2_scratch) {
-        c->l2_scratch_bytes = (size_t)256 << 20;      // 256 MiB > 126 MB L2
+        c->l2_scratch_bytes = (size_t)256 << 20;      // 256 MiB > 50 MB L2
         BM_CUDA(cudaMalloc(&c->l2_scratch, c->l2_scratch_bytes));
     }
     BM_CUDA(cudaMemsetAsync(c->l2_scratch, 0, c->l2_scratch_bytes, c->stream));

@@ -430,7 +430,7 @@ struct Dbm : DbmBase {
             BM_CUDA(cudaMemsetAsync(flag.p, 0, sizeof(unsigned int), ctx->stream));
             for (int i = 0; i < L; ++i) {
                 const size_t n = (size_t)rows * Hs[i];
-                max_abs_diff_kernel<T><<<148, 256, 0, ctx->stream>>>(cur[i], nxt[i], n, flag.p);
+                max_abs_diff_kernel<T><<<ctx->sm_count, 256, 0, ctx->stream>>>(cur[i], nxt[i], n, flag.p);
                 count_launch(ctx);
             }
             allreduce_max_u32(ctx, flag.p, 1);           // sharded rows: every rank runs the same number of sweeps
@@ -692,7 +692,7 @@ int bm_dbm_create(bm_ctx* hctx, const bm_dbm_cfg* cfg, bm_dbm** out) {
     BM_REQUIRE(cfg->n_particles > 0 && cfg->batch_size > 0, "n_particles and batch_size must be positive");
     BM_REQUIRE(cfg->v_kind != BM_UNIT_GAUSSIAN || cfg->sigma, "gaussian visible layer needs sigma");
     BM_CUDA(cudaSetDevice(ctx->device));
-    // BM_COMPUTE_BF16 (opt-in): float32 models with Bernoulli hidden layers run their GEMMs on tcgen05; every other
+    // BM_COMPUTE_BF16 (opt-in): float32 models with Bernoulli hidden layers run their GEMMs on the tensor cores; every other
     // combination keeps the storage-precision CUDA-core engine (as bm_rbm_create does for unit kinds the
     // tensor-core epilogue does not implement)
     DbmBase* d;

@@ -2,10 +2,10 @@
 //
 // Same state, same update kernels and same control flow as Dbm<float> (the reference's dbm.py, see the
 // header of bm_dbm.cu); every GEMM -- the layer-wise Gibbs step with its two-sided input
-// H_{i-1} W_i + H_{i+1} W_{i+1}^T (dbm.py:385-427) as ONE two-pair tcgen05 op, the mean-field sweeps
+// H_{i-1} W_i + H_{i+1} W_{i+1}^T (dbm.py:385-427) as ONE two-pair tensor-core op, the mean-field sweeps
 // (:429-478), the particle sweeps (:480-509), the gradients pos^T mu - neg^T h (:558-568, split over the
 // batch rows), the pre-activations of the AIS ladder (:650-736) -- runs on the fused tensor-core layer op
-// of bm_tc.cu (bf16 operands, fp32 accumulation in TMEM, bias + beta scaling + sigmoid + Philox draw in
+// of bm_tc.cu (bf16 operands, fp32 accumulation in registers, bias + beta scaling + sigmoid + Philox draw in
 // the epilogue).  Variables stay fp32 as in the reference; activations (variational parameters, particles,
 // AIS states) are kept as bf16 operands, binary samples being exact in bf16.  AIS pre-activations leave the
 // kernel in fp32 and the importance weights are accumulated in fp64 from differences
@@ -236,7 +236,7 @@ struct DbmTC : Dbm<float> {
             for (DevBuf<bf16_t>* b : {&Wb[i], &mu_b[i], &mu2_b[i], &h_b[i], &h2_b[i]}) b->zero(ctx->stream);
         }
         // default: persistent dataflow programs -- 5 speculated mean-field sweeps per launch, the committed particle sweeps
-        // as one launch (cfg4 on the B200: 1.56 ms/step with one launch per op, 1.06 ms with programs); = 0: one launch per op
+        // as one launch; = 0: one launch per op
         { const char* e = getenv("BM_DBM_MF_CHUNK"); mf_chunk = e ? atoi(e) : 5; }
         { const char* e = getenv("BM_DBM_PCD_PROGRAM"); pcd_program = e ? atoi(e) != 0 : true; }
         { const char* e = getenv("BM_DBM_TC_MIXED"); mixed_layouts = e && atoi(e) != 0; }
@@ -415,7 +415,7 @@ struct DbmTC : Dbm<float> {
             launch_tc_program(ctx, *pslot, RngKey{}, 0);
             BM_CUDA(cudaMemsetAsync(mf_flags.p, 0, (size_t)c * sizeof(unsigned int), ctx->stream));
             for (int i = 0; i < L; ++i) {
-                mf_chunk_diffs_kernel<<<dim3(74, c), 256, 0, ctx->stream>>>(hist[i].p, (size_t)B * ldn[i + 1], ldn[i + 1], rows, Hs[i], mf_flags.p);
+                mf_chunk_diffs_kernel<<<dim3((unsigned)(ctx->sm_count / 2), c), 256, 0, ctx->stream>>>(hist[i].p, (size_t)B * ldn[i + 1], ldn[i + 1], rows, Hs[i], mf_flags.p);
                 count_launch(ctx);
             }
             allreduce_max_u32(ctx, mf_flags.p, (size_t)c);       // sharded rows: the same sweep index on every rank
@@ -455,7 +455,7 @@ struct DbmTC : Dbm<float> {
         while (step < max_mf) {
             BM_CUDA(cudaMemsetAsync(flag.p, 0, sizeof(unsigned int), ctx->stream));
             for (int i = 0; i < L; ++i) {
-                max_abs_diff_bf16_kernel<<<148, 256, 0, ctx->stream>>>(cur[i], ldn[i + 1], nxt[i], ldn[i + 1], rows, Hs[i], flag.p);
+                max_abs_diff_bf16_kernel<<<ctx->sm_count, 256, 0, ctx->stream>>>(cur[i], ldn[i + 1], nxt[i], ldn[i + 1], rows, Hs[i], flag.p);
                 count_launch(ctx);
             }
             allreduce_max_u32(ctx, flag.p, 1);

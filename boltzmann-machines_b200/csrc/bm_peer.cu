@@ -178,11 +178,9 @@ __global__ void __launch_bounds__(256) dp_scatter_kernel(const __grid_constant__
 }
 
 // ---- the same two kernels with the transfers as BULK asynchronous copies (shared memory -> peer global memory) -------------
-// An experiment (BM_PEER_BULK=1), kept for the record: event profile of the store version on 4 B200s (profiles/r02_notes.md): push
-// 30 us, update 40 us for 2.4 MB / 6 MB to the peers.  Here a block sums / updates whole rows into shared memory and one thread
-// hands them to the copy engine of its SM (cp.async.bulk.global.shared::cta: one transaction of n_hidden * 4 bytes per row and
-// destination), the local copy included.  Parity green on 2 GPUs, but slower than the stores (push 26 us, update 30 us at N = 2):
-// the exchange is bound by its two system-scope publish / wait hops and kernel boundaries, not by the stores' granularity.
+// An alternative (BM_PEER_BULK=1, off by default): a block sums / updates whole rows into shared memory and one thread hands
+// them to the copy engine of its SM (cp.async.bulk.global.shared::cta: one transaction of n_hidden * 4 bytes per row and
+// destination), the local copy included.  Its speed against the plain stores is not measured on H100s.
 __device__ __forceinline__ uint32_t peer_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void bulk_store(void* gdst, const void* ssrc, uint32_t bytes) {
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(peer_smem_u32(ssrc)), "r"(bytes) : "memory");
@@ -457,8 +455,7 @@ void PeerExchange::run(DpStep& s) {
         ++prof_n; prof_pending = false;
     }
     if (prof) BM_CUDA(cudaEventRecord(ev[0], ctx->stream));
-    // BM_PEER_BULK=1: transfers as bulk asynchronous copies from shared memory.  Measured (profiles/r02_notes.md): NOT faster --
-    // 2 GPUs: 0.2185 ms/step against 0.1902 with plain 16-byte stores (push 26 us, update 30 us) -- so the default stays off.
+    // BM_PEER_BULK=1: transfers as bulk asynchronous copies from shared memory (not measured on H100s; off by default).
     static const int bulk_env = [] { const char* e = getenv("BM_PEER_BULK"); return e ? atoi(e) : 0; }();
     const bool bulk = bulk_env != 0 && H % 8 == 0 && (size_t)H * 4 * 2 + (size_t)H * 2 <= 96 * 1024;
     const int r0 = ctx->rank * rows_per;
@@ -493,7 +490,7 @@ void PeerExchange::run(DpStep& s) {
     const size_t items = r1 > r0 ? (size_t)(r1 - r0) * H / 4 : 0;
     const unsigned w_blocks = (unsigned)((items + 255) / 256);
     // BM_PEER_SPLIT=1: the update writes this rank's copy only and a second, full-width kernel copies the rows out to the peers
-    // (measured at 4 GPUs: no gain -- the limit is the rate of 16-byte peer stores, not the number of blocks issuing them)
+    // (off by default; not measured on H100s)
     static const int split_env = [] { const char* e = getenv("BM_PEER_SPLIT"); return e ? atoi(e) : 0; }();
     const bool split = ctx->nranks > 1 && split_env != 0;
     dp_update_kernel<<<w_blocks + (unsigned)((nb + 255) / 256), 256, 0, ctx->stream>>>(s, w_blocks, split ? 1 : 0);

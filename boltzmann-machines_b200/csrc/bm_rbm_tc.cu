@@ -2,7 +2,7 @@
 //
 // Variables (W, biases, momentum accumulators, q_means) stay in fp32 exactly as in the
 // reference; every GEMM of the CD-k step -- h0, the 2k chain half-steps and the fused
-// positive-minus-negative dW -- runs on tcgen05 with bf16 operands and fp32 accumulation, as ONE
+// positive-minus-negative dW -- runs on the tensor cores (wgmma) with bf16 operands and fp32 accumulation, as ONE
 // persistent dataflow launch (bm_tc.cu: TcProgram).  Activations live in L2/HBM as bf16 only
 // (binary samples are exact in bf16).  A bf16 shadow of W is refreshed by the weight-update
 // kernel.  Metrics (free energy / PLL) are evaluated in fp32 by the inherited CUDA-core kernels.
@@ -41,7 +41,7 @@ struct RbmTC : RbmSimt<float> {
     // column statistics of base_rbm.py:453,457 cost no pass of their own.  sum(X - v_k) (:451) is two more ops of the
     // program ([V x 1] = X^T 1 - v_k^T 1).  Everything is summed and applied by ONE kernel (launch_cd_tail).
     // The constant columns sit at VP = V rounded up to 64, i.e. behind the last 64-column box a TMA store of the visible
-    // activations can touch (observed on the B200: a store box that is clipped by the tensor edge inside a 16-byte unit
+    // activations can touch (seen on an earlier GPU: a store box that is clipped by the tensor edge inside a 16-byte unit
     // overwrites the rest of that unit).  Rows V .. VP-1 of the statistics are don't-cares.
     int VP() const { return (V + 63) / 64 * 64; }
     int VM() const { return VP() + 2; }
@@ -283,9 +283,10 @@ struct RbmTC : RbmSimt<float> {
                 g.split_stride = vstride(); g.ld_f32 = 1;
                 return g;
             };
-            // The positive statistics depend on the input and h0 only.  When the chain leaves CTA pairs idle (cfg2: 64 units
-            // per half-step on 74 pairs) and is long enough to hide them, they run on those pairs BESIDE the chain and only the
-            // negative ones are left for the end of the step.
+            // The positive statistics depend on the input and h0 only.  When the chain leaves CTA pairs idle and is long enough
+            // to hide them, they run on those pairs BESIDE the chain and only the negative ones are left for the end of the step.
+            // The cycle counts below (per K chunk of a statistics unit, per chain half-step) are rough estimates carried over
+            // from an earlier GPU; they are not measured on the H100.
             if (prog.chain_units < 0)            // shapes are fixed per cached program: plan once
                 for (const TcGemm& o : ops) prog.chain_units = std::max(prog.chain_units, tc_plan_units(ctx, o));
             const int chain_units = prog.chain_units;

@@ -1,32 +1,31 @@
-// Fused "layer ops" on the 5th-generation tensor cores (sm_100a only), as a persistent
+// Fused "layer ops" on the Hopper tensor cores (sm_90a: wgmma + TMA + mbarrier), as a persistent
 // multi-phase dataflow kernel.
 //
-//   C[M,N] = sum_p (+/-) A_p * B_p^T          bf16 operands, fp32 accumulation in TMEM
+//   C[M,N] = sum_p (+/-) A_p * B_p^T          bf16 operands, fp32 accumulation in registers
 //   out    = sample(act(acc_scale * C * sigma + bias_scale * bias))
 //
 // One such op replaces, per Gibbs half-step, the reference's tf.matmul + 3 element-wise kernels +
 // the random_uniform/Less/Cast sampling chain (rbm/base_rbm.py:329-365, layers.py:34-51); the dW op
 // replaces the two gradient GEMMs (base_rbm.py:447-448) by ONE GEMM over the concatenated batch
-// dimension whose negative phase is subtracted by the MMA's a_negate bit.  A *program* strings the
+// dimension whose negative phase is subtracted by the MMA's scale-a = -1.  A *program* strings the
 // 2k+1 half-steps of a CD-k chain and its dW into one launch: units (op, row-block pair, column
 // block) are walked in a fixed global order by all CTA pairs and start as soon as the row blocks they
 // read are complete (per-row-block counters in global memory), so nothing waits on a kernel boundary,
 // and the epilogue of one half-step overlaps the MMAs of the next.  Activations pass between ops
-// through L2-resident bf16 buffers (8 MB at batch 4096: never evicted to HBM by the 126 MB L2).
+// through L2-resident bf16 buffers (8 MB at batch 4096, well inside the 50 MB L2).
 //
-// Per CTA (384 threads, one CTA per SM; CL = 2: CTA pairs, tcgen05 cta_group::2, 256-row tiles):
-//   warp 0     TMA producer: the warp's lanes issue the 2-6 bulk-tensor copies of a stage in one
-//              instruction; 128B-swizzled tiles; mbarrier ring of 6 x 32 KiB (pair) / 4 x 48 KiB
-//   warp 1     MMA issuer (pair leader only): one thread issues tcgen05.mma kind::f16, M=128/256, N<=256, K=16
-//   warp 2     TMEM allocator (512 columns = 2 accumulator stages)
-//   warps 4-11 epilogue: tcgen05.ld 32x32b.x32 (thread = one accumulator row, 32 columns), bias,
-//              sigmoid by ex2/rcp, Philox-4x32-10 in registers, bf16/fp32 stores; then the unit's
-//              completion is published (fence + atomic) for the ops that read it.
-// Why pairs: one SM ingests only ~50 B/clk from L2 (measured), a 128x256 tile needs 96 B/clk at full
-// MMA rate; with cta_group::2 each SM loads its 128 A rows and HALF of the B tile (64 B/clk).
-// Operand layouts: K-major and MN-major shared-memory descriptors are both used so that a single
-// bf16 copy of W serves v->h (W as MN-major B) and h->v (W as K-major B) and no activation is ever
-// transposed in memory (dW takes X and h as MN-major A and B).
+// Per CTA (384 threads, one CTA per SM, 128-row tiles; a "pair" is two CTAs that own the two
+// 128-row blocks of a 256-row group -- a scheduling unit of the dataflow, the CTAs share nothing):
+//   warps 0-7  two consumer warpgroups: warpgroup g issues wgmma m64n64k16 for tile rows 64g..64g+63
+//              (one instruction per 64-column block of the tile and one for a last 16/32/48-column block, accumulators in registers), then runs
+//              the epilogue on its accumulators: bias, sigmoid by ex2/rcp, Philox-4x32-10 in registers,
+//              bf16 outputs into a 128B-swizzled staging FIFO, fp32 outputs straight to global memory
+//   warp 11    TMA producer: 128B-swizzled tiles, mbarrier ring of 3 x 48 KiB (BN = 256) to 6 x 24 KiB (BN = 64) stages
+//   warps 9-10 publishers: TMA-store the staged bf16 granules and publish them (fence + atomic)
+//              for the ops that read them
+// Operand layouts: K-major and MN-major shared-memory descriptors are both used (wgmma's transpose
+// bits) so that a single bf16 copy of W serves v->h (W as MN-major B) and h->v (W as K-major B) and no
+// activation is ever transposed in memory (dW takes X and h as MN-major A and B).
 #include "bm_tc.h"
 #include "bm_tc_desc.h"
 #include <cuda.h>
@@ -40,27 +39,30 @@
 
 namespace bm {
 
-constexpr int BM = 128;            // rows per CTA tile = TMEM lanes
+constexpr int BM = 128;            // rows per CTA tile (two warpgroups x 64)
 constexpr int BK = 64;             // K per pipeline stage = one 128-byte swizzle atom of bf16
+constexpr int MAX_BN = 256;        // accumulator columns per tile: up to 4 x 32 fp32 registers per consumer thread
+constexpr int NB_MAX = MAX_BN / 64;
+// Register split between the warpgroups (setmaxnreg): the producer warpgroup (TMA, publishers) gives registers to the two
+// consumer warpgroups, whose 128 accumulator registers at BN = 256 would not fit the launch's 168.  The CTA keeps the registers
+// it was launched with (168 x 384): a split that asks for more leaves setmaxnreg.inc waiting for ever.
+constexpr int PRODUCER_REGS = 56, CONSUMER_REGS = 224;
 constexpr int MAX_STAGES = 10;
-constexpr int ACC_STAGES = 2;
-constexpr int ACC_COLS = 256;      // TMEM columns per accumulator stage
+constexpr int ACC_STAGES = 2;      // per-unit barriers and bias slices are double-buffered
 constexpr int A_BYTES = BM * BK * 2;           // 16 KiB
-constexpr int B_BYTES = 256 * BK * 2;          // 32 KiB (BN <= 256)
-constexpr int RING_BYTES = 160 * 1024;                // 5 x 32 KiB pair stages / 3 x 48 KiB single-CTA stages
+constexpr int RING_BYTES = 160 * 1024;                // 3 x 48 KiB stages (BN = 256) ... 6 x 24 KiB (BN = 64)
 constexpr int N_OUT_BUF = 4;                          // bf16 output staging FIFO: 64-column x 128-row granules
 constexpr int OUT_BUF_BYTES = BM * 64 * 2;            // 16 KiB each, 128B-swizzled like the operand tiles
 constexpr int OUT_BYTES = N_OUT_BUF * OUT_BUF_BYTES;
-constexpr int SMEM_BARRIER_BYTES = 320;   // full/empty ring, tfull/tempty, TMEM slot, unit/granule barriers
+constexpr int SMEM_BARRIER_BYTES = 320;   // full/empty ring, tempty, unit/granule barriers
 constexpr int GRAN_COLS = 64;             // bf16 outputs leave the SM (and are published) in 64-column granules
-constexpr int EPI_WARPS = 16;        // 4 per TMEM lane quarter: the epilogue is latency-bound, it needs warps
-constexpr int EPI_SUBS = EPI_WARPS / 4;
-constexpr int CW = 16;               // accumulator columns per epilogue chunk (one tcgen05.ld.x16)
-constexpr int TC_THREADS = 32 * (4 + EPI_WARPS);
+constexpr int CONSUMER_THREADS = 256;
+constexpr int CONSUMER_WARPS = CONSUMER_THREADS / 32;
+constexpr int TC_THREADS = CONSUMER_THREADS + 128;
+constexpr int LAUNCH_REGS = 65536 / TC_THREADS / 8 * 8;   // per thread under __launch_bounds__(TC_THREADS, 1): 168
 // Warp roles.  The SM's issue arbiter prefers the highest warp id: the single-thread roles whose latency
-// is on the critical path (TMA producer, MMA issuer, publishers) get the highest ids so that sixteen busy
-// (or spinning) epilogue warps cannot starve them.
-constexpr int W_PUB0 = EPI_WARPS, W_PUB1 = EPI_WARPS + 1, W_MMA = EPI_WARPS + 2, W_TMA = EPI_WARPS + 3;
+// is on the critical path (TMA producer, publishers) get the highest ids.  Warp 8 has no role.
+constexpr int W_PUB0 = 9, W_PUB1 = 10, W_TMA = 11;
 
 enum : int {
     MODE_GENERIC = 0,                // every combination, flags read at run time
@@ -75,20 +77,21 @@ enum : int {
 };
 
 constexpr int MAX_PHASES = 96;
-// The series form of the AIS increment (chunk_body, MODE_AIS_UNITS) is used for ladders of >= 400 temperatures: with
+// The series form of the AIS increment (pair_body, MODE_AIS_UNITS) is used for ladders of >= 400 temperatures: with
 // t = (b - a) z and d = (next - (a + b) / 2) z its errors are t^2/24 sigma''/sigma (midpoint rule) and d^4/24 sigma''''/sigma
 // (third-order series) relative to the term -- < 3e-6 and < 1e-8 for |z| <= 10 at these spacings, and both vanish with
 // sigma' for large |z|.  Coarser ladders take the closed form (MODE_AIS_UNITS_G).
 constexpr float AIS_MAX_CT = 2.5e-3f, AIS_MAX_CD = 4.0e-3f;
-constexpr int SBIAS_BYTES = ACC_STAGES * 256 * (int)sizeof(float);
+constexpr int SBIAS_BYTES = ACC_STAGES * MAX_BN * (int)sizeof(float);
 
 constexpr int SMEM_BYTES = RING_BYTES + OUT_BYTES + SMEM_BARRIER_BYTES + SBIAS_BYTES;     // 231,744 of 232,448
 
 // The ops of the running launch.  Constant memory on purpose: indexed by warp-uniform values it is read
 // through the uniform datapath, so the TMA / MMA issue loops keep their descriptors, coordinates and
-// trip counts in uniform registers -- with per-thread registers every UTMALDG / UTCHMMA is wrapped in
-// an ELECT + R2UR "waterfall" loop of ~100 cycles, which made the issue loops the bottleneck.
+// trip counts in uniform registers.
 __constant__ TcPhaseLite c_ph[MAX_PHASES];
+static_assert(PRODUCER_REGS * 128 + CONSUMER_REGS * CONSUMER_THREADS <= LAUNCH_REGS * TC_THREADS,
+              "the setmaxnreg split must fit the registers the CTA is launched with");
 
 
 // ------------------------------------------------------------------------------------------
@@ -106,8 +109,8 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 // Every wait of the kernel is bounded: a wait that has not been satisfied after HANG_NS of wall time (a lost
-// arrival, a peer that never launched, stale dataflow counters) traps -- the launch fails with an error instead
-// of holding the GPU for ever.  The clock is only read every 4096 failed attempts.
+// arrival, stale dataflow counters) traps -- the launch fails with an error instead of holding the GPU for
+// ever.  The clock is only read every 4096 failed attempts.
 constexpr unsigned long long HANG_NS = 4000000000ull;
 __device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 __device__ __forceinline__ void hang_guard(uint32_t& n, unsigned long long& t0) {
@@ -132,8 +135,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         hang_guard(n, t0);
     }
 }
-// for waits that are expected to be long (epilogue warps waiting for an accumulator or a staging
-// buffer): sleep between attempts instead of spinning in the issue slots of the busy roles
+// for waits that are expected to be long (consumers waiting for a staging buffer): sleep between attempts
+// instead of spinning in the issue slots of the busy roles
 __device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity, uint32_t ns = 128) {
     const uint32_t addr = smem_u32(bar);
     uint32_t done;
@@ -155,13 +158,6 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, uint64_t map, uint32_t
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
-// cta_group::2 loads: data lands in the issuing CTA, the transaction bytes are counted on the
-// LEADER CTA's mbarrier (address with the peer bit cleared)
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t dst, uint64_t map, uint32_t leader_bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(dst), "l"(map), "r"(leader_bar), "r"(c0), "r"(c1) : "memory");
-}
 __device__ __forceinline__ void tma_store_2d(uint64_t map, uint32_t src, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                  ::"l"(map), "r"(src), "r"(c0), "r"(c1) : "memory");
@@ -169,34 +165,19 @@ __device__ __forceinline__ void tma_store_2d(uint64_t map, uint32_t src, int c0,
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void sts128(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+__device__ __forceinline__ void sts32(uint32_t addr, uint32_t a) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(a) : "memory");
 }
 // release: everything this thread has observed (completed bulk stores, barrier-acquired stores of the
-// epilogue warps) is visible to whoever acquires the counter
+// consumer warps) is visible to whoever acquires the counter
 __device__ __forceinline__ void red_release_add(int* p, int v) {
     asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-    asm volatile(
-        "{\n\t"
-        ".reg .b32 remAddr32;\n\t"
-        "mapa.shared::cluster.u32 remAddr32, %0, %1;\n\t"
-        "mbarrier.arrive.shared::cluster.b64 _, [remAddr32];\n\t"
-        "}" ::"r"(smem_u32(bar)), "r"(cta) : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ uint32_t cluster_id_x() { uint32_t r; asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r)); return r; }
-__device__ __forceinline__ uint32_t cluster_count_x() { uint32_t r; asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)map) : "memory");
 }
 // One lane of a converged warp (elect.sync): unlike `lane == 0`, ptxas knows that exactly one thread
-// executes the guarded code and moves its operands to uniform registers without an ELECT/R2UR loop.
+// executes the guarded code and moves its operands to uniform registers.
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred = 0;
     asm volatile(
@@ -211,71 +192,145 @@ __device__ __forceinline__ bool elect_one() {
 #define DBG_MARK(slot) do { if (L.dbg && blockIdx.x == 0) L.dbg[(slot)] = (unsigned long long)clock64(); } while (0)
 // per-unit marks of CTA 0: slot 64 + ord * 8 + kind (ord = ordinal of the unit within this CTA, < 24)
 #define DBG_UNIT(kind, ord) do { if (L.dbg && blockIdx.x == 0 && (ord) < 24) L.dbg[64 + (ord) * 8 + (kind)] = (unsigned long long)clock64(); } while (0)
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// descriptors are passed as (lo, hi) halves: only `lo` (the start address) changes between MMAs
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                          uint32_t idesc, uint32_t accumulate) {
+// ---- wgmma ---------------------------------------------------------------------------------
+// every warp of a warpgroup executes one of them, at the top of its role's branch
+__device__ __forceinline__ void regs_to_consumers() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS)); }
+__device__ __forceinline__ void regs_from_producers() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS)); }
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D[64xN] (+)= (+/-A)[64x16] * B[16xN], N = 16, 32, 48 or 64: bf16 operands from shared memory, fp32 accumulator fragment `d`
+// (thread t of the warpgroup holds rows 16 (t/32) + (t%32)/4 (+8) and columns 8 i + 2 (t%4) (+1), registers 4 i .. 4 i + 3).
+// TA / TB: the operand is MN-major (wgmma transpose bit); NEG: scale-a = -1.
+template <int TA, int TB, int NEG>
+__device__ __forceinline__ void wgmma_n16(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t"
-        "}" ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate) : "memory");
+        "setp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+        "%8, %9, p, %11, 1, %12, %13;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(NEG ? -1 : 1), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                              uint32_t idesc, uint32_t accumulate) {
+template <int TA, int TB, int NEG>
+__device__ __forceinline__ void wgmma_n32(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %5, p;\n\t"
-        "}" ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate) : "memory");
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p, %19, 1, %20, %21;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(NEG ? -1 : 1), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {      // arrives on `bar` in both CTAs of the pair
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
+template <int TA, int TB, int NEG>
+__device__ __forceinline__ void wgmma_n48(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %26, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, "
+        "%24, %25, p, %27, 1, %28, %29;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(NEG ? -1 : 1), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+template <int TA, int TB, int NEG>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, %35, 1, %36, %37;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(NEG ? -1 : 1), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+template <int N, int TA, int TB, int NEG>
+__device__ __forceinline__ void wgmma_m64nk16(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+    if constexpr (N == 16) wgmma_n16<TA, TB, NEG>(d, da, db, scale_d);
+    else if constexpr (N == 32) wgmma_n32<TA, TB, NEG>(d, da, db, scale_d);
+    else if constexpr (N == 48) wgmma_n48<TA, TB, NEG>(d, da, db, scale_d);
+    else wgmma_n64<TA, TB, NEG>(d, da, db, scale_d);
+}
 
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout): start address [0,14),
-// leading byte offset [16,30), stride byte offset [32,46) (all >> 4), version=1 at bit 46,
-// layout type SWIZZLE_128B = 2 at bits [61,64).
+// Shared-memory matrix descriptor (wgmma): start address [0,14), leading byte offset [16,30), stride byte
+// offset [32,46) (all >> 4), layout type SWIZZLE_128B = 1 at bits [62,64).
 //   K-major tile  [rows][64 k] : 8-row groups are 1024 B apart (SBO); LBO unused.
 //   MN-major tile [64 k][64 mn] boxes of 8 KiB: 64-wide MN blocks are 8192 B apart (LBO),
 //                 8-k groups 1024 B apart (SBO).
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, int mn_major) {
     const uint64_t lbo = mn_major ? (8192u >> 4) : 1u;
     const uint64_t sbo = 1024u >> 4;
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (lbo << 16) | (sbo << 32) | (1ull << 46) | (2ull << 61);
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (lbo << 16) | (sbo << 32) | (1ull << 62);
+}
+
+// One K chunk (64) of the warpgroup's 64 x BN accumulator, BN = 16 BN16: 4 K=16 steps x (BN / 64 blocks of 64 columns + a
+// last block of BN % 64), as one wgmma group.  The A rows of warpgroup g and the B columns of block j both sit 8 KiB apart in
+// either layout (one 64-row / 64-column box each), and a K=16 step advances 32 B (K-major, inside the swizzle atom) or 2 KiB
+// (MN-major, two 8-k groups).  Every run-time choice is a template argument: a wgmma on a path ptxas cannot prove
+// warpgroup-uniform is serialised.
+template <int TA, int TB, int NEG, int BN16>
+__device__ __forceinline__ void mma_chunk(float (&acc)[NB_MAX][32], uint32_t sA, uint32_t sB, uint32_t first) {
+    constexpr int NB = BN16 / 4, TAIL = 16 * (BN16 % 4);
+    const uint32_t a_step = TA ? 2048u : 32u, b_step = TB ? 2048u : 32u;
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t da = make_smem_desc(sA + (uint32_t)k * a_step, TA);
+        const uint32_t scale_d = (first && k == 0) ? 0u : 1u;
+#pragma unroll
+        for (int j = 0; j < NB; ++j)
+            wgmma_m64nk16<64, TA, TB, NEG>(acc[j], da, make_smem_desc(sB + (uint32_t)j * 8192u + (uint32_t)k * b_step, TB), scale_d);
+        if constexpr (TAIL > 0)
+            wgmma_m64nk16<(TAIL > 0 ? TAIL : 64), TA, TB, NEG>(acc[NB < NB_MAX ? NB : 0], da,
+                                                             make_smem_desc(sB + (uint32_t)NB * 8192u + (uint32_t)k * b_step, TB), scale_d);
+    }
+    wg_commit();
+}
+// cfg = (A MN-major) << 2 | (B MN-major) << 1 | negated; BN a multiple of 16 (of 64 when B is MN-major), at most 256
+template <int C>
+__device__ __forceinline__ void mma_chunk_cfg(int bn16, float (&acc)[NB_MAX][32], uint32_t sA, uint32_t sB, uint32_t first) {
+    constexpr int TA = (C >> 2) & 1, TB = (C >> 1) & 1, NEG = C & 1;
+    if constexpr (TB) {
+        switch (bn16) {
+            case 4: mma_chunk<TA, TB, NEG, 4>(acc, sA, sB, first); break;
+            case 8: mma_chunk<TA, TB, NEG, 8>(acc, sA, sB, first); break;
+            case 12: mma_chunk<TA, TB, NEG, 12>(acc, sA, sB, first); break;
+            default: mma_chunk<TA, TB, NEG, 16>(acc, sA, sB, first); break;
+        }
+    } else {
+        switch (bn16) {
+#define BM_MMA_CASE(W) case W: mma_chunk<TA, TB, NEG, W>(acc, sA, sB, first); break;
+            BM_MMA_CASE(1) BM_MMA_CASE(2) BM_MMA_CASE(3) BM_MMA_CASE(4) BM_MMA_CASE(5) BM_MMA_CASE(6) BM_MMA_CASE(7)
+            BM_MMA_CASE(8) BM_MMA_CASE(9) BM_MMA_CASE(10) BM_MMA_CASE(11) BM_MMA_CASE(12) BM_MMA_CASE(13) BM_MMA_CASE(14)
+            BM_MMA_CASE(15)
+#undef BM_MMA_CASE
+            default: mma_chunk<TA, TB, NEG, 16>(acc, sA, sB, first); break;
+        }
+    }
+}
+__device__ __forceinline__ void mma_chunk_any(int cfg, int bn16, float (&acc)[NB_MAX][32], uint32_t sA, uint32_t sB, uint32_t first) {
+    switch (cfg) {
+        case 0: mma_chunk_cfg<0>(bn16, acc, sA, sB, first); break;
+        case 1: mma_chunk_cfg<1>(bn16, acc, sA, sB, first); break;
+        case 2: mma_chunk_cfg<2>(bn16, acc, sA, sB, first); break;
+        case 3: mma_chunk_cfg<3>(bn16, acc, sA, sB, first); break;
+        case 4: mma_chunk_cfg<4>(bn16, acc, sA, sB, first); break;
+        case 5: mma_chunk_cfg<5>(bn16, acc, sA, sB, first); break;
+        case 6: mma_chunk_cfg<6>(bn16, acc, sA, sB, first); break;
+        default: mma_chunk_cfg<7>(bn16, acc, sA, sB, first); break;
+    }
 }
 
 __device__ __forceinline__ float fast_softplus(float x) { return fmaxf(x, 0.f) + __logf(1.0f + __expf(-fabsf(x))); }
@@ -293,18 +348,13 @@ __device__ __forceinline__ float u32_to_one_two(uint32_t w, uint32_t mant_mask, 
     asm("lop3.b32 %0, %1, %2, %3, 0xEA;" : "=r"(bits) : "r"(w), "r"(mant_mask), "r"(one_bits));
     return __uint_as_float(bits);
 }
-// 256-bit store (sm_100+): a thread's 8 consecutive fp32 go out as one full 32-byte sector
-__device__ __forceinline__ void stg256(float* dst, const float (&v)[8]) {
-    asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                 ::"l"(dst), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7]) : "memory");
-}
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
     __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
     return *reinterpret_cast<uint32_t*>(&h2);
 }
-// Polling uses relaxed loads: an acquire load makes ptxas emit CCTL.IVALL (a full L1 invalidation) on
-// every iteration, which evicted the epilogue warps' bias/constant lines for as long as a producer
-// warp was waiting.  One acquire fence follows the successful poll.
+// Polling uses relaxed loads: an acquire load makes ptxas emit a full L1 invalidation on every iteration,
+// which evicted the consumer warps' bias/constant lines for as long as a producer warp was waiting.  One
+// acquire fence follows the successful poll.
 __device__ __forceinline__ int ld_acquire(const int* p) {
     int v; asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v;
 }
@@ -326,16 +376,14 @@ template <int MODE> struct EpiCfg {
     static constexpr bool f32 = (MODE == MODE_RAW_F32);
 };
 
-// the epilogue's view of a phase, copied into registers once per unit (the descriptor itself lives in
-// global memory; reading it inside the element loops would put L2 latency on every use)
+// the epilogue's view of a phase, copied into registers once per unit
 struct EpiPhase {
     int M, N, BN, act, sample;
     float acc_scale, bias_scale;
-    const float* __restrict__ bias;
     const float* __restrict__ sigma;
     const float* __restrict__ noise_sigma;
-    __nv_bfloat16* __restrict__ out_mean_bf;  int ld_mean_bf;
-    __nv_bfloat16* __restrict__ out_state_bf; int ld_state_bf;
+    __nv_bfloat16* __restrict__ out_mean_bf;
+    __nv_bfloat16* __restrict__ out_state_bf;
     float* __restrict__ out_f32;              int ld_f32;
     unsigned long long split_stride;
     float ais_a, ais_b, ais_next, ais_lin;
@@ -345,25 +393,18 @@ struct EpiPhase {
 struct EpiCtx {
     EpiPhase p;
     RngKey rng;
-    int m, n_blk, split;          // this thread's global row, the tile's column block and K split
-    uint32_t t_row;               // TMEM address of this thread's lane, column 0 of the accumulator stage
-    uint64_t* tempty;             // accumulator-free barrier (leader's in pair mode)
-    int sub, lane;                // sub: which chunks (mod EPI_SUBS) this warp takes
+    int m0;                       // global row of this thread's first accumulator row (the second is m0 + 8)
+    int r0;                       // the same row inside the 128-row tile
+    int n_blk, split;             // the tile's column block and K split
+    int lane;
     const float* sbias;           // shared memory: bias_scale * bias (x -log2 e for sigmoid) of the tile's columns
-    bool remote_arrive;           // pair mode, peer CTA: signal the leader's barrier
-    // bf16 outputs are staged in shared memory and leave the SM as TMA stores (publisher warp)
     uint32_t out_base;            // shared address of the staging FIFO
-    uint32_t row_off;             // this thread's row inside a staging buffer: (row % 128) * 128 bytes
-    uint32_t row_swz;             // row & 7: XOR pattern of the 128-byte swizzle
-    uint64_t* out_full;           // [N_OUT_BUF] a staged granule is complete (16 warp arrivals)
+    uint64_t* out_full;           // [N_OUT_BUF] a staged granule is complete (8 warp arrivals)
     uint64_t* out_free;           // [N_OUT_BUF] its TMA store has read the buffer (publisher)
-    uint32_t* seq;                // FIFO position (same sequence in every warp and in the publisher)
+    uint32_t* seq;                // FIFO position (same sequence in every consumer warp and in the publishers)
     uint32_t mant_mask, one_bits; // TcLaunch::mant_mask / one_bits
 };
 
-// One CW-column chunk of one accumulator row: activation, sampling, then
-//   bf16 means / states -> this thread's row of the staging buffers (two 16-byte units each),
-//   fp32 -> global memory directly (dW partials and raw pre-activations only).
 // softplus(b z) - softplus(a z) = log1p(sigmoid(a z) * expm1((b - a) z)) without cancellation (b - a ~ 1e-3): short series
 // where both arguments are small (the common case), the library functions elsewhere
 __device__ __forceinline__ float ais_softplus_diff(float a, float b, float z) {
@@ -377,165 +418,141 @@ __device__ __forceinline__ float ais_softplus_diff(float a, float b, float z) {
     return log1pf(y);
 }
 
-// AIS_UNITS only: the chunk's contribution to the row's log-weight; AIS_STATE: sum of state * pre-scaled bias; else 0
+// Two adjacent accumulator columns (n, n + 1; n even) of one row m: activation, sampling, packed bf16 mean / state and the
+// fp32 store.  wf / ws are the Philox words of the two columns: words 2 (n % 4 / 2) and 2 (n % 4 / 2) + 1 of the row's
+// block n / 4 -- the same draws, column for column, as a thread that owns the whole block.
+// Returns the pair's contribution to the row's AIS log-weight (AIS modes) or 0.
 template <int MODE>
-__device__ __forceinline__ float chunk_body(const EpiCtx& c, const uint32_t (&v)[CW], int ch, int n0, int n_valid,
-                                            uint32_t smem_mean, uint32_t smem_state, bool store_ok) {
+__device__ __forceinline__ float pair_body(const EpiCtx& c, float v0, float v1, uint32_t wf, uint32_t ws, float b0, float b1,
+                                           int n, int m, bool row_ok, float* out_f32, bool f32_vec,
+                                           uint32_t& mean_pk, uint32_t& state_pk) {
     typedef EpiCfg<MODE> E;
     const EpiPhase& p = c.p;
     float ais_part = 0.f;
     const int act = E::fixed ? E::act : p.act;
     const int smp = (MODE == MODE_AIS_UNITS || MODE == MODE_AIS_UNITS_S) ? SMP_BERNOULLI :
                     (E::fixed && MODE != MODE_AIS_UNITS_G) ? E::sample : p.sample;
-    float* const out_f32 = ((E::fixed && !E::f32) || !p.out_f32) ? nullptr : p.out_f32 + (size_t)c.split * p.split_stride;
     // fold the sigmoid's -log2(e) into the affine map of the accumulator
     const float a_s = (act == ACT_SIGMOID) ? p.acc_scale * -1.4426950408889634f : p.acc_scale;
     const bool has_sigma = !E::fixed && p.sigma != nullptr;
-    const int m = c.m;
-    // in the fixed modes which outputs exist is known at compile time (no per-group branches)
-    const bool do_mean = E::fixed ? E::mean_bf : (p.out_mean_bf != nullptr);
-    const bool do_state = (MODE == MODE_AIS_UNITS || MODE == MODE_AIS_UNITS_S) ? true :
-                          (E::fixed && MODE != MODE_AIS_UNITS_G) ? E::state_bf : (p.out_state_bf != nullptr);
     const bool do_f32 = E::fixed ? E::f32 : (out_f32 != nullptr);
-    const bool f32_vec = n_valid == CW && (p.ld_f32 & 3) == 0;       // rows 16-byte aligned, whole chunk
-    // rows 32-byte aligned (row pitch, split stride and base): one full sector per store instruction and thread
-    const bool f32_wide = f32_vec && (p.ld_f32 & 7) == 0 && (p.split_stride & 7) == 0 &&
-                          (reinterpret_cast<uintptr_t>(p.out_f32) & 31) == 0;
-    float f32_prev[4] = {0.f, 0.f, 0.f, 0.f};
-    uint32_t mean_pk[CW / 2], state_pk[CW / 2];
+    const float v[2] = {v0, v1};
+    const float bq[2] = {b0, b1};
+    const uint32_t words[2] = {wf, ws};
+    float g[2] = {0.f, 0.f};
+    if (!E::fixed && smp == SMP_GAUSSIAN) {
+        const float u1 = fmaxf(u32_to_unit_float(wf), 1.0e-7f);
+        const float r = sqrtf(-2.0f * __logf(u1));
+        float s, co;
+        __sincosf(6.2831853071795864769f * u32_to_unit_float(ws), &s, &co);
+        g[0] = s * r; g[1] = co * r;
+    }
+    float mu[2], st[2];
 #pragma unroll
-    for (int q = 0; q < CW / 4; ++q) {
-        const float4 b4 = *reinterpret_cast<const float4*>(c.sbias + ch * CW + q * 4);   // broadcast LDS.128
-        const float bq[4] = {b4.x, b4.y, b4.z, b4.w};
-        U4 w{0, 0, 0, 0};
-        if (smp != SMP_NONE) w = site_block(c.rng, (uint32_t)m, (uint32_t)((n0 >> 2) + q));
-        const uint32_t words[4] = {w.x, w.y, w.z, w.w};
-        float g[4] = {0.f, 0.f, 0.f, 0.f};
-        if (!E::fixed && smp == SMP_GAUSSIAN) {
-            const float u1a = fmaxf(u32_to_unit_float(w.x), 1.0e-7f), u1b = fmaxf(u32_to_unit_float(w.z), 1.0e-7f);
-            const float ra = sqrtf(-2.0f * __logf(u1a)), rb = sqrtf(-2.0f * __logf(u1b));
-            float sa, ca, sb, cb;
-            __sincosf(6.2831853071795864769f * u32_to_unit_float(w.y), &sa, &ca);
-            __sincosf(6.2831853071795864769f * u32_to_unit_float(w.w), &sb, &cb);
-            g[0] = sa * ra; g[1] = ca * ra; g[2] = sb * rb; g[3] = cb * rb;
+    for (int j = 0; j < 2; ++j) {
+        const bool valid = n + j < p.N;
+        float x = a_s * v[j];
+        if (has_sigma && valid) x *= p.sigma[n + j];
+        x += bq[j];
+        float m_ = x;
+        float s_;
+        if (MODE == MODE_AIS_UNITS || MODE == MODE_AIS_UNITS_S) {
+            // x = z (acc_scale = bias_scale = 1).  p = sigmoid(beta_next z) serves the draw AND the weight increment:
+            //   softplus(b z) - softplus(a z) = int_a^b z sigmoid(beta z) dbeta = t sigmoid(m z)  (+ t^3 z^-2 ... / 24: < 1e-7 t)
+            //   with t = (b - a) z, m = (a + b) / 2, and sigmoid(m z) = sigmoid(beta_next z - d), d = (beta_next - m) z, as its
+            //   third-order series in d around p (error terms: AIS_MAX_CT / AIS_MAX_CD above).
+            float e_, p_;
+            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e_) : "f"(x * p.ais_next * -1.4426950408889634f));
+            asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(p_) : "f"(1.0f + e_));
+            s_ = ((u32_to_one_two(words[j], c.mant_mask, c.one_bits) - 1.0f) < p_) ? 1.0f : 0.0f;
+            if (MODE == MODE_AIS_UNITS) {
+                const float q_ = fmaf(-p_, p_, p_);                                 // sigma1 = p (1 - p)
+                const float d_ = p.ais_cd * x;
+                const float s2 = fmaf(-2.0f, p_, 1.0f);                             // sigma2 / sigma1
+                const float s3 = fmaf(-6.0f, q_, 1.0f);                             // sigma3 / sigma1
+                const float in = fmaf(-d_ * (1.0f / 3.0f), s3, s2);
+                const float sm = fmaf(-d_ * q_, fmaf(-0.5f * d_, in, 1.0f), p_);    // sigmoid(m z)
+                ais_part = fmaf(valid ? p.ais_ct * x : 0.f, sm, ais_part);
+            }
+            mu[j] = 0.f; st[j] = s_;
+            continue;
         }
-        float mu[4], st[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int e = q * 4 + j;
-            float x = a_s * __uint_as_float(v[e]);
-            if (has_sigma && e < n_valid) x *= p.sigma[n0 + e];
-            x += bq[j];
-            float m_ = x;
-            float s_;
-            if (MODE == MODE_AIS_UNITS || MODE == MODE_AIS_UNITS_S) {
-                // x = z (acc_scale = bias_scale = 1).  p = sigmoid(beta_next z) serves the draw AND the weight increment:
-                //   softplus(b z) - softplus(a z) = int_a^b z sigmoid(beta z) dbeta = t sigmoid(m z)  (+ t^3 z^-2 ... / 24: < 1e-7 t)
-                //   with t = (b - a) z, m = (a + b) / 2, and sigmoid(m z) = sigmoid(beta_next z - d), d = (beta_next - m) z, as its
-                //   third-order series in d around p (error terms: AIS_MAX_CT / AIS_MAX_CD above).
-                float e_, p_;
-                asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e_) : "f"(x * p.ais_next * -1.4426950408889634f));
-                asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(p_) : "f"(1.0f + e_));
-                s_ = ((u32_to_one_two(words[j], c.mant_mask, c.one_bits) - 1.0f) < p_) ? 1.0f : 0.0f;
-                if (MODE == MODE_AIS_UNITS) {
-                    const float q_ = fmaf(-p_, p_, p_);                                 // sigma1 = p (1 - p)
-                    const float d_ = p.ais_cd * x;
-                    const float s2 = fmaf(-2.0f, p_, 1.0f);                             // sigma2 / sigma1
-                    const float s3 = fmaf(-6.0f, q_, 1.0f);                             // sigma3 / sigma1
-                    const float in = fmaf(-d_ * (1.0f / 3.0f), s3, s2);
-                    const float sm = fmaf(-d_ * q_, fmaf(-0.5f * d_, in, 1.0f), p_);    // sigmoid(m z)
-                    ais_part = fmaf((e < n_valid) ? p.ais_ct * x : 0.f, sm, ais_part);
-                }
-                mu[j] = 0.f; st[j] = s_;
-                continue;
-            }
-            if (MODE == MODE_AIS_UNITS_G) {
-                // any temperatures, optional sampling / output: the closed forms
-                if (p.ais_logw && e < n_valid) ais_part += ais_softplus_diff(p.ais_a, p.ais_b, x);
-                float e_;
-                asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e_) : "f"(x * p.ais_next * -1.4426950408889634f));
-                const float d_ = 1.0f + e_;
-                if (smp == SMP_BERNOULLI) {
-                    const float u12 = u32_to_one_two(words[j], c.mant_mask, c.one_bits);
-                    s_ = (fmaf(u12, d_, -d_) < 1.0f) ? 1.0f : 0.0f;
-                } else {
-                    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(s_) : "f"(d_));
-                }
-                mu[j] = 0.f; st[j] = s_;
-                continue;
-            }
-            if (MODE == MODE_SIG_BERN_STATE || MODE == MODE_AIS_STATE) {
-                // only the draw is needed: u < 1/(1+e)  <=>  u*(1+e) < 1, with u = u12 - 1 folded into one FMA
-                // (no reciprocal, no "- 1.0f"); e = inf (p = 0) gives NaN -> 0, e = 0 (p = 1) gives u < 1 -> 1
-                float e_;
-                asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e_) : "f"(x));
-                const float d_ = 1.0f + e_;
+        if (MODE == MODE_AIS_UNITS_G) {
+            // any temperatures, optional sampling / output: the closed forms
+            if (p.ais_logw && valid) ais_part += ais_softplus_diff(p.ais_a, p.ais_b, x);
+            float e_;
+            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e_) : "f"(x * p.ais_next * -1.4426950408889634f));
+            const float d_ = 1.0f + e_;
+            if (smp == SMP_BERNOULLI) {
                 const float u12 = u32_to_one_two(words[j], c.mant_mask, c.one_bits);
                 s_ = (fmaf(u12, d_, -d_) < 1.0f) ? 1.0f : 0.0f;
-                mu[j] = 0.f; st[j] = s_;
-                if (MODE == MODE_AIS_STATE && e < n_valid) ais_part = fmaf(s_, bq[j], ais_part);
-                continue;
+            } else {
+                asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(s_) : "f"(d_));
             }
-            if (act == ACT_SIGMOID) m_ = sigmoid_from_neg_log2(x);
-            else if (!E::fixed && act == ACT_SOFTPLUS) m_ = fast_softplus(x);
-            s_ = m_;
-            if (smp == SMP_BERNOULLI) s_ = ((u32_to_one_two(words[j], c.mant_mask, c.one_bits) - 1.0f) < m_) ? 1.0f : 0.0f;
-            else if (!E::fixed && smp == SMP_GAUSSIAN)
-                s_ = m_ + ((p.noise_sigma && e < n_valid) ? p.noise_sigma[n0 + e] : 1.0f) * g[j];
-            mu[j] = m_; st[j] = s_;
+            mu[j] = 0.f; st[j] = s_;
+            continue;
         }
-        if (do_mean) { mean_pk[2 * q] = pack_bf16(mu[0], mu[1]); mean_pk[2 * q + 1] = pack_bf16(mu[2], mu[3]); }
-        if (do_state) { state_pk[2 * q] = pack_bf16(st[0], st[1]); state_pk[2 * q + 1] = pack_bf16(st[2], st[3]); }
-        if (do_f32 && store_ok) {
-            float* dst = out_f32 + (size_t)m * p.ld_f32 + n0 + q * 4;
-            if (f32_wide) {                       // 32-byte stores: every other group carries the previous one with it
-                if (q & 1) { const float v8[8] = {f32_prev[0], f32_prev[1], f32_prev[2], f32_prev[3], mu[0], mu[1], mu[2], mu[3]}; stg256(dst - 4, v8); }
-                else { f32_prev[0] = mu[0]; f32_prev[1] = mu[1]; f32_prev[2] = mu[2]; f32_prev[3] = mu[3]; }
-            } else if (f32_vec) *reinterpret_cast<float4*>(dst) = make_float4(mu[0], mu[1], mu[2], mu[3]);
-            else {
-#pragma unroll
-                for (int j = 0; j < 4; ++j) if (q * 4 + j < n_valid) dst[j] = mu[j];
-            }
+        if (MODE == MODE_SIG_BERN_STATE || MODE == MODE_AIS_STATE) {
+            // only the draw is needed: u < 1/(1+e)  <=>  u*(1+e) < 1, with u = u12 - 1 folded into one FMA
+            // (no reciprocal, no "- 1.0f"); e = inf (p = 0) gives NaN -> 0, e = 0 (p = 1) gives u < 1 -> 1
+            float e_;
+            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e_) : "f"(x));
+            const float d_ = 1.0f + e_;
+            const float u12 = u32_to_one_two(words[j], c.mant_mask, c.one_bits);
+            s_ = (fmaf(u12, d_, -d_) < 1.0f) ? 1.0f : 0.0f;
+            mu[j] = 0.f; st[j] = s_;
+            if (MODE == MODE_AIS_STATE && valid) ais_part = fmaf(s_, bq[j], ais_part);
+            continue;
         }
+        if (act == ACT_SIGMOID) m_ = sigmoid_from_neg_log2(x);
+        else if (!E::fixed && act == ACT_SOFTPLUS) m_ = fast_softplus(x);
+        s_ = m_;
+        if (smp == SMP_BERNOULLI) s_ = ((u32_to_one_two(words[j], c.mant_mask, c.one_bits) - 1.0f) < m_) ? 1.0f : 0.0f;
+        else if (!E::fixed && smp == SMP_GAUSSIAN)
+            s_ = m_ + ((p.noise_sigma && valid) ? p.noise_sigma[n + j] : 1.0f) * g[j];
+        mu[j] = m_; st[j] = s_;
     }
-    // columns past N and rows past M are written to the staging buffer too: the TMA store clips them
-    const uint32_t u0 = (uint32_t)((ch * CW) & 63) >> 3;           // first 16-byte unit of this chunk in the 128-byte row
-#pragma unroll
-    for (int i = 0; i < CW / 8; ++i) {
-        const uint32_t off = c.row_off + (((u0 + (uint32_t)i) ^ c.row_swz) << 4);
-        if (do_mean) sts128(smem_mean + off, mean_pk[4 * i], mean_pk[4 * i + 1], mean_pk[4 * i + 2], mean_pk[4 * i + 3]);
-        if (do_state) sts128(smem_state + off, state_pk[4 * i], state_pk[4 * i + 1], state_pk[4 * i + 2], state_pk[4 * i + 3]);
+    mean_pk = pack_bf16(mu[0], mu[1]);
+    state_pk = pack_bf16(st[0], st[1]);
+    if (do_f32 && row_ok) {
+        float* dst = out_f32 + (size_t)m * p.ld_f32 + n;
+        if (f32_vec && n + 1 < p.N) *reinterpret_cast<float2*>(dst) = make_float2(mu[0], mu[1]);
+        else {
+            if (n < p.N) dst[0] = mu[0];
+            if (n + 1 < p.N) dst[1] = mu[1];
+        }
     }
     return ais_part;
 }
 
-// One warp's share of a tile: TMEM lane quarter (warp % 4) x the CW-column chunks ch = sub (mod EPI_SUBS).
-// All warps sweep the tile left to right together, granule (64 columns) by granule: each granule of each
-// bf16 output takes the next buffer of the staging FIFO, is written by the 16 warps and announced on the
-// buffer's `full` barrier; the publisher warp stores it with TMA and publishes it to the other SMs.
-template <int MODE, bool PAIR>
-__device__ __forceinline__ void epilogue_tile(const EpiCtx& c) {
+// The warpgroup's share of a tile, granule (64 columns = one accumulator block) by granule: each granule of each bf16
+// output takes the next buffer of the staging FIFO, is written by the 8 consumer warps and announced on the buffer's
+// `full` barrier; the publisher warps store it with TMA and publish it to the other SMs.
+template <int MODE>
+__device__ __forceinline__ void epilogue_tile(const EpiCtx& c, const float (&acc)[NB_MAX][32]) {
     typedef EpiCfg<MODE> E;
     const EpiPhase& p = c.p;
-    const int BN = p.BN;
-    const int n_chunks = BN / CW;                  // BN is a multiple of 16
-    const bool row_ok = c.m < p.M;
+    const int nb = (p.BN + GRAN_COLS - 1) / GRAN_COLS;     // the last block may be 16, 32 or 48 columns wide (fp32 outputs only)
     const bool do_mean = E::fixed ? E::mean_bf : (p.out_mean_bf != nullptr);
     const bool do_state = (MODE == MODE_AIS_UNITS || MODE == MODE_AIS_UNITS_S) ? true :
                           (E::fixed && MODE != MODE_AIS_UNITS_G) ? E::state_bf : (p.out_state_bf != nullptr);
-    float ais_sum = 0.f;
-    int last_ch = -1;
-    for (int ch = c.sub; ch < n_chunks; ch += EPI_SUBS) last_ch = ch;
-    if (last_ch < 0) {          // this warp has no chunk in the tile: release the accumulator at once
-        __syncwarp();
-        if (c.lane == 0) {
-            if (PAIR && c.remote_arrive) { if constexpr (PAIR) mbar_arrive_remote(c.tempty, 0); } else mbar_arrive(c.tempty);
-        }
-    }
-    constexpr int gc = GRAN_COLS / CW;             // chunks per granule
-    const int n_gran = (n_chunks + gc - 1) / gc;
+    const int smp = (MODE == MODE_AIS_UNITS || MODE == MODE_AIS_UNITS_S) ? SMP_BERNOULLI :
+                    (E::fixed && MODE != MODE_AIS_UNITS_G) ? E::sample : p.sample;
+    float* const out_f32 = ((E::fixed && !E::f32) || !p.out_f32) ? nullptr : p.out_f32 + (size_t)c.split * p.split_stride;
+    // float2 stores: even row pitch, split stride and 8-byte aligned base
+    const bool f32_vec = (p.ld_f32 & 1) == 0 && (p.split_stride & 1) == 0 && (reinterpret_cast<uintptr_t>(p.out_f32) & 7) == 0;
+    const int lane = c.lane, q = lane & 3;
+    const int m1 = c.m0 + 8;
+    const bool ok0 = c.m0 < p.M, ok1 = m1 < p.M;
+    const bool odd = (lane & 1) != 0;
+    // rows r0 and r0 + 8 share their position inside the 128-byte swizzle pattern (r & 7 = lane / 4)
+    const uint32_t swz = (uint32_t)(lane >> 2) & 7u;
+    const uint32_t off0 = (uint32_t)c.r0 * 128u + (uint32_t)q * 4u, off1 = off0 + 8u * 128u;
+    float ais0 = 0.f, ais1 = 0.f;
     uint32_t seq = *c.seq;
-    for (int g = 0; g < n_gran; ++g) {
+#pragma unroll
+    for (int j = 0; j < NB_MAX; ++j) {
+        if (j >= nb) break;
         uint32_t smem_mean = 0, smem_state = 0;
         int b_mean = 0, b_state = 0;
         if (do_mean) {
@@ -548,27 +565,39 @@ __device__ __forceinline__ void epilogue_tile(const EpiCtx& c) {
             mbar_wait_relaxed(&c.out_free[b_state], ((seq / N_OUT_BUF) & 1u) ^ 1u);
             smem_state = c.out_base + (uint32_t)b_state * OUT_BUF_BYTES; ++seq;
         }
-        const int ch_end = min(n_chunks, (g + 1) * gc);
-        for (int ch = g * gc + c.sub; ch < ch_end; ch += EPI_SUBS) {
-            uint32_t v[CW];
-            __syncwarp();                            // tcgen05.ld is warp-collective (.sync.aligned)
-            tmem_ld16(c.t_row + (uint32_t)(ch * CW), v);
-            tmem_ld_wait();
-            if (ch == last_ch) {
-                // all of this warp's reads of the accumulator are done: hand it back to the MMA warp
-                tc_fence_before();
-                __syncwarp();
-                if (c.lane == 0) {
-                    if (PAIR && c.remote_arrive) { if constexpr (PAIR) mbar_arrive_remote(c.tempty, 0); } else mbar_arrive(c.tempty);
+        const int col0 = c.n_blk * p.BN + j * GRAN_COLS;
+        const int gcols = min(GRAN_COLS, p.BN - j * GRAN_COLS);
+        if (col0 < p.N) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                if (8 * i >= gcols) break;
+                const int cl = 8 * i + 2 * q;                    // column inside the granule
+                const int n = col0 + cl;
+                // Philox: the lane pair (q even, q odd) shares the 4-column block n / 4 of rows m0 and m0 + 8.  The even
+                // lane draws the block of m0, the odd lane that of m0 + 8, and they swap the halves the other one needs.
+                uint32_t w0f = 0, w0s = 0, w1f = 0, w1s = 0;
+                if (smp != SMP_NONE) {
+                    const U4 w = site_block(c.rng, (uint32_t)(odd ? m1 : c.m0), (uint32_t)(n >> 2));
+                    const uint32_t give_f = odd ? w.x : w.z, give_s = odd ? w.y : w.w;
+                    const uint32_t got_f = __shfl_xor_sync(0xffffffffu, give_f, 1);
+                    const uint32_t got_s = __shfl_xor_sync(0xffffffffu, give_s, 1);
+                    if (!odd) { w0f = w.x; w0s = w.y; w1f = got_f; w1s = got_s; }
+                    else { w0f = got_f; w0s = got_s; w1f = w.z; w1s = w.w; }
                 }
+                const float2 b2 = *reinterpret_cast<const float2*>(c.sbias + j * GRAN_COLS + cl);
+                uint32_t mp0, sp0, mp1, sp1;
+                ais0 += pair_body<MODE>(c, acc[j][4 * i], acc[j][4 * i + 1], w0f, w0s, b2.x, b2.y, n, c.m0, ok0, out_f32, f32_vec, mp0, sp0);
+                ais1 += pair_body<MODE>(c, acc[j][4 * i + 2], acc[j][4 * i + 3], w1f, w1s, b2.x, b2.y, n, m1, ok1, out_f32, f32_vec, mp1, sp1);
+                // columns past N and rows past M are written to the staging buffer too: the TMA store clips them
+                const uint32_t u = (((uint32_t)i ^ swz) << 4);
+                if (do_mean) { sts32(smem_mean + off0 + u, mp0); sts32(smem_mean + off1 + u, mp1); }
+                if (do_state) { sts32(smem_state + off0 + u, sp0); sts32(smem_state + off1 + u, sp1); }
             }
-            const int n0 = c.n_blk * BN + ch * CW;
-            if (n0 < p.N) ais_sum += chunk_body<MODE>(c, v, ch, n0, min(CW, p.N - n0), smem_mean, smem_state, row_ok);
         }
         if (do_mean || do_state) {
             fence_proxy_async_smem();                // this thread's staging writes -> visible to the TMA unit
             __syncwarp();
-            if (c.lane == 0) {
+            if (lane == 0) {
                 if (do_mean) mbar_arrive(&c.out_full[b_mean]);
                 if (do_state) mbar_arrive(&c.out_full[b_state]);
             }
@@ -576,10 +605,13 @@ __device__ __forceinline__ void epilogue_tile(const EpiCtx& c) {
     }
     *c.seq = seq;
     if constexpr (E::ais) {
-        // this thread's share of its row's log-weight: fp64 atomics (four threads per row and column tile)
-        if (p.ais_logw && row_ok) {
-            const double inc = (double)(MODE == MODE_AIS_STATE ? ais_sum * p.ais_lin : ais_sum);
-            asm volatile("red.global.add.f64 [%0], %1;" ::"l"(p.ais_logw + c.m), "d"(inc) : "memory");     // (no return value wanted)
+        // the row's log-weight increment: the four lanes of a row sum their columns, one fp64 atomic per row and tile
+        ais0 += __shfl_xor_sync(0xffffffffu, ais0, 1); ais0 += __shfl_xor_sync(0xffffffffu, ais0, 2);
+        ais1 += __shfl_xor_sync(0xffffffffu, ais1, 1); ais1 += __shfl_xor_sync(0xffffffffu, ais1, 2);
+        if (p.ais_logw && q == 0) {
+            const float s = MODE == MODE_AIS_STATE ? p.ais_lin : 1.0f;
+            if (ok0) asm volatile("red.global.add.f64 [%0], %1;" ::"l"(p.ais_logw + c.m0), "d"((double)(ais0 * s)) : "memory");
+            if (ok1) asm volatile("red.global.add.f64 [%0], %1;" ::"l"(p.ais_logw + m1), "d"((double)(ais1 * s)) : "memory");
         }
     }
 }
@@ -615,21 +647,20 @@ __device__ __forceinline__ UnitInfo decode_unit(const TcPhaseLite* ph, int local
     return u;
 }
 
+// CL = 2: CTAs 2c and 2c + 1 take row blocks 2g and 2g + 1 of row group g of every unit of pair c; CL = 1: one CTA per
+// row block (single-op launches with one row block).
 template <int CL>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_program_kernel(const __grid_constant__ TcLaunch L) {
-    constexpr bool pair = (CL == 2);
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = smem_raw;                      // [operand ring | output staging FIFO | barriers | bias]
     if ((smem_u32(smem) & 1023u) != 0) __trap();   // 128B-swizzle atoms need 1024-byte alignment
     uint8_t* const out_stage = smem + RING_BYTES;
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + RING_BYTES + OUT_BYTES);
     uint64_t* empty = full + MAX_STAGES;
-    uint64_t* tfull = empty + MAX_STAGES;
-    uint64_t* tempty = tfull + ACC_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + ACC_STAGES);
-    uint64_t* unit_bar = tempty + ACC_STAGES + 1;                 // [ACC_STAGES] all epilogue warps stored the unit
-    uint64_t* out_full = unit_bar + ACC_STAGES;                   // [N_OUT_BUF] staged granule written by all epilogue warps
+    uint64_t* tempty = empty + MAX_STAGES;                        // [ACC_STAGES] the publishers are done with the unit's stage
+    uint64_t* unit_bar = tempty + ACC_STAGES;                     // [ACC_STAGES] all consumer warps stored the unit
+    uint64_t* out_full = unit_bar + ACC_STAGES;                   // [N_OUT_BUF] staged granule written by all consumer warps
     uint64_t* out_free = out_full + N_OUT_BUF;                    // [N_OUT_BUF] staged granule read by its TMA store
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -638,42 +669,22 @@ tc_program_kernel(const __grid_constant__ TcLaunch L) {
     const TcPhase* const gph = L.n_phases ? L.phases : &L.inl;      // tensor maps (global / parameter memory)
     if (warp == W_TMA && lane == 0) {
         tma_prefetch_desc(&gph->tmA[0]); tma_prefetch_desc(&gph->tmB[0]);
-    }
-    if (warp == W_MMA && lane == 0) {
-        // pair: the leader's `full` collects its own expect_tx-arrive and the peer's arrive; its `tempty`
-        // collects the epilogue warps of both CTAs; `empty`/`tfull` get one multicast commit each
-        for (int s = 0; s < L.stages; ++s) { mbar_init(&full[s], (uint32_t)CL); mbar_init(&empty[s], 1); }
-        // tempty: the epilogue warps and the two publisher warps of both CTAs
-        for (int a = 0; a < ACC_STAGES; ++a) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], (uint32_t)((EPI_WARPS + 2) * CL)); }
-        for (int a = 0; a < ACC_STAGES; ++a) mbar_init(&unit_bar[a], EPI_WARPS);
-        for (int b = 0; b < N_OUT_BUF; ++b) { mbar_init(&out_full[b], EPI_WARPS); mbar_init(&out_free[b], 1); }
+        for (int s = 0; s < L.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }   // empty: both consumer warpgroups
+        for (int a = 0; a < ACC_STAGES; ++a) { mbar_init(&tempty[a], 2); mbar_init(&unit_bar[a], CONSUMER_WARPS); }
+        for (int b = 0; b < N_OUT_BUF; ++b) { mbar_init(&out_full[b], CONSUMER_WARPS); mbar_init(&out_free[b], 1); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == W_PUB0) {
-        if constexpr (pair) {        // one warp of each CTA of the pair allocates collectively
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::);
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-        }
-    }
-    tc_fence_before();
-    if constexpr (pair) cluster_sync_all(); else __syncthreads();   // peers' barriers must exist before any remote arrive
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    __syncthreads();
     if (threadIdx.x == 0) DBG_MARK(1);
 
     const int n_ops = L.n_phases ? L.n_phases : 1;
-    // clusters are (2,1,1): rank = blockIdx.x & 1, cluster id = blockIdx.x >> 1 (kept as expressions of
-    // blockIdx / gridDim so that the compiler knows they are warp-uniform)
-    const int crank = pair ? (int)(blockIdx.x & 1u) : 0;
-    const int cid = pair ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
+    // (kept as expressions of blockIdx so that the compiler knows they are warp-uniform)
+    const int crank = CL == 2 ? (int)(blockIdx.x & 1u) : 0;
+    const int cid = CL == 2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
 
     if (warp == W_TMA) {
         // ================================ TMA producer =====================================
-        // The whole warp walks the K chunks; for each chunk lane 0 arms the barrier and lanes
-        // 0..n_ops-1 issue one bulk-tensor copy each in the same warp instruction.
+        regs_to_consumers();
         int stage = 0; uint32_t phase = 0;
         int pi = 0, ul = -1;
         int ord = -1;
@@ -686,11 +697,9 @@ tc_program_kernel(const __grid_constant__ TcLaunch L) {
             // this op's tensor maps -> descriptor cache while the unit still waits for its inputs
             if ((L.flags & 8) && lane < 2 * ph->n_pairs) tma_prefetch_desc(lane & 1 ? &gp->tmB[lane >> 1] : &gp->tmA[lane >> 1]);
             const int BN = ph->BN;
-            const int half_bn = BN >> 1;
-            const uint32_t tx_bytes = pair ? 2u * (A_BYTES + (uint32_t)half_bn * BK * 2) : A_BYTES + (uint32_t)BN * BK * 2;
-            const int b_cols = pair ? half_bn : BN;          // B columns this CTA fetches
+            const uint32_t tx_bytes = A_BYTES + (uint32_t)BN * BK * 2;
             const int m_blk = u.m_group * CL + crank;
-            const int n_col0 = u.n_blk * BN + (pair ? crank * half_bn : 0);
+            const int n_col0 = u.n_blk * BN;
             // ---- dataflow: wait until the row blocks this unit reads have been written ----------
             if (ph->n_deps > 0) {
                 if (lane == 0) {
@@ -730,7 +739,7 @@ tc_program_kernel(const __grid_constant__ TcLaunch L) {
                 b_c0[pr] = b_mn[pr] ? n_col0 : 0;
                 b_c1[pr] = b_mn[pr] ? 0 : n_col0;
             }
-            const int nB_mn = b_cols >> 6;            // 64-column boxes of an MN-major B tile
+            const int nB_mn = BN >> 6;                // 64-column boxes of an MN-major B tile
             const uint32_t smem_base = smem_u32(smem);
             const bool ordered = cdep != nullptr;
             int fenced_upto = u.c_begin;         // K positions [c_begin, fenced_upto) are known ready and fenced
@@ -759,18 +768,16 @@ tc_program_kernel(const __grid_constant__ TcLaunch L) {
                             hang_guard(hn, ht0);
                         }
                         fenced_upto = ci + ready_prefix;
-                        if (L.dbg && blockIdx.x == 0 && ord == 1 && lane == 0 && ci - u.c_begin < 20) { L.dbg[456 + ci - u.c_begin] = (unsigned long long)clock64(); L.dbg[480 + ci - u.c_begin] = (unsigned long long)fenced_upto; }
                         // acquire the producers' stores, then order them before this unit's TMA reads (async proxy)
                         if (!(L.flags & 1)) asm volatile("fence.acq_rel.gpu;" ::: "memory");
                         // The producers' data was written by TMA stores and is read here by TMA loads (the same
                         // proxy); only the counter travels through the generic proxy.  flags bit 1 narrows the
                         // cross-proxy fence to the global state space, bit 2 drops it (the TMA issue below is
                         // control-dependent on the acquired counter value) -- a full fence.proxy.async also waits
-                        // for this thread's own in-flight bulk copies (~1.2 k cycles per poll, measured).
+                        // for this thread's own in-flight bulk copies.
                         if (L.flags & 4) {}
                         else if (L.flags & 2) asm volatile("fence.proxy.async.global;" ::: "memory");
                         else asm volatile("fence.proxy.async;" ::: "memory");
-                        if (L.dbg && blockIdx.x == 0 && ord == 1 && lane == 0 && ci - u.c_begin < 20) L.dbg[432 + ci - u.c_begin] = (unsigned long long)clock64();
                     }
                 }
                 const int pr = (c >= chunks0) ? 1 : 0;
@@ -785,106 +792,25 @@ tc_program_kernel(const __grid_constant__ TcLaunch L) {
                 if (elect_one()) {               // one thread issues; every operand above is warp-uniform
                     if (ci - u.c_begin < 24 && (L.n_phases == 0 || ord == 1)) DBG_MARK(8 + (ci - u.c_begin));
                     const uint32_t fbar = smem_u32(&full[stage]);
-                    if constexpr (pair) {
-                        // both CTAs load their own A rows and their half of the B tile; bytes are counted on the leader
-                        const uint32_t lbar = fbar & 0xFEFFFFFFu;
-                        if (crank == 0) mbar_expect_tx(&full[stage], tx_bytes); else mbar_arrive_remote(&full[stage], 0);
-                        if (!amn) tma_load_2d_2sm(sA, mA, lbar, kc, ac1);
-                        else { tma_load_2d_2sm(sA, mA, lbar, ac0, ac1 + kc); tma_load_2d_2sm(sA + 8192u, mA, lbar, ac0 + 64, ac1 + kc); }
-                        if (!bmn) tma_load_2d_2sm(sB, mB, lbar, kc, bc1);
-                        else for (int j = 0; j < nB_mn; ++j) tma_load_2d_2sm(sB + (uint32_t)j * 8192u, mB, lbar, bc0 + j * 64, kc);
-                    } else {
-                        mbar_expect_tx(&full[stage], tx_bytes);
-                        if (!amn) tma_load_2d(sA, mA, fbar, kc, ac1);
-                        else { tma_load_2d(sA, mA, fbar, ac0, ac1 + kc); tma_load_2d(sA + 8192u, mA, fbar, ac0 + 64, ac1 + kc); }
-                        if (!bmn) tma_load_2d(sB, mB, fbar, kc, bc1);
-                        else for (int j = 0; j < nB_mn; ++j) tma_load_2d(sB + (uint32_t)j * 8192u, mB, fbar, bc0 + j * 64, kc);
-                    }
-                }
-                if (++stage == L.stages) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp == W_MMA) {
-        // ================================ MMA issuer (the pair's leader CTA only) ============
-        // The whole warp runs the loop converged (all values warp-uniform -> uniform registers);
-        // lane 0 issues the tcgen05 instructions.
-        if (crank == 0) {
-            int stage = 0; uint32_t phase = 0;
-            int acc = 0; uint32_t acc_phase = 0;
-            int pi = 0, ul = -1;
-            int ord = -1;
-            const uint32_t smem_base = smem_u32(smem);
-            while (walk_next(pi, ul, cid, n_ops)) {
-                ++ord;
-                const TcPhaseLite* ph = &c_ph[pi];
-                const UnitInfo u = decode_unit(ph, ul);
-                // instruction descriptor (cute::UMMA::InstrDescriptor): D=f32 [4,6), A=bf16 [7,10), B=bf16 [10,13),
-                // a_negate 13, a_major 15, b_major 16, N>>3 [17,23), M>>4 [24,29)
-                const uint32_t idesc_base = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(ph->BN >> 3) << 17) |
-                                            ((uint32_t)((pair ? 2 * BM : BM) >> 4) << 24);
-                // per operand pair: instruction descriptor, K=16 slice strides and the constant upper
-                // halves of the shared-memory descriptors -- the chunk loop only adds addresses
-                uint32_t idesc_p[2], a_step_p[2], b_step_p[2], a_hi_p[2], b_hi_p[2], a_lo_p[2], b_lo_p[2];
-#pragma unroll
-                for (int pr = 0; pr < 2; ++pr) {
-                    const int a_mn = ph->a_mn[pr], b_mn = ph->b_mn[pr];
-                    idesc_p[pr] = idesc_base | ((uint32_t)ph->a_neg[pr] << 13) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16);
-                    a_step_p[pr] = a_mn ? (2048u >> 4) : (32u >> 4);    // descriptor units (16 B) per K=16 slice
-                    b_step_p[pr] = b_mn ? (2048u >> 4) : (32u >> 4);
-                    const uint64_t da = make_smem_desc(0, a_mn), db = make_smem_desc(0, b_mn);
-                    a_hi_p[pr] = (uint32_t)(da >> 32); a_lo_p[pr] = (uint32_t)da;
-                    b_hi_p[pr] = (uint32_t)(db >> 32); b_lo_p[pr] = (uint32_t)db;
-                }
-                const int chunks0 = ph->chunks[0];
-                const bool ordered = ph->dep_chunk_ctr != nullptr;
-                mbar_wait(&tempty[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * ACC_COLS);
-                uint32_t accumulate = 0;
-                for (int ci = u.c_begin; ci < u.c_end; ++ci) {
-                    const int c = ordered ? (int)ph->k_order[ci] : ci;     // same order as the producer warp
-                    const int pr = (c >= chunks0) ? 1 : 0;
-                    const uint32_t idesc = pr ? idesc_p[1] : idesc_p[0];
-                    const uint32_t a_step = pr ? a_step_p[1] : a_step_p[0], b_step = pr ? b_step_p[1] : b_step_p[0];
-                    const uint32_t a_hi = pr ? a_hi_p[1] : a_hi_p[0], b_hi = pr ? b_hi_p[1] : b_hi_p[0];
-                    const uint32_t aaddr = smem_base + (uint32_t)stage * (uint32_t)L.stage_bytes;
-                    // operand addresses are < 256 KiB: the 14-bit start-address field (16-byte units) never carries
-                    const uint32_t a_lo = (pr ? a_lo_p[1] : a_lo_p[0]) | ((aaddr & 0x3FFFFu) >> 4);
-                    const uint32_t b_lo = (pr ? b_lo_p[1] : b_lo_p[0]) | (((aaddr + A_BYTES) & 0x3FFFFu) >> 4);
-                    mbar_wait(&full[stage], phase);
-                    tc_fence_after();
-                    if (elect_one()) {
-                        if (ci == u.c_begin) DBG_UNIT(2, ord);
-                        if (ci - u.c_begin < 24 && (L.n_phases == 0 || ord == 1)) DBG_MARK(32 + (ci - u.c_begin));
-#pragma unroll
-                        for (int k = 0; k < BK / 16; ++k) {
-                            if constexpr (pair) umma_bf16_2sm(d_tmem, a_lo + k * a_step, a_hi, b_lo + k * b_step, b_hi, idesc, accumulate);
-                            else umma_bf16(d_tmem, a_lo + k * a_step, a_hi, b_lo + k * b_step, b_hi, idesc, accumulate);
-                            accumulate = 1;
-                        }
-                        // the smem slot is free once these MMAs retire (both CTAs' producers are told)
-                        if constexpr (pair) umma_commit_2sm(&empty[stage]); else umma_commit(&empty[stage]);
-                    }
-                    accumulate = 1;
-                    if (++stage == L.stages) { stage = 0; phase ^= 1; }
-                }
-                if (elect_one()) {
-                    if constexpr (pair) umma_commit_2sm(&tfull[acc]); else umma_commit(&tfull[acc]);   // accumulator complete -> epilogue
-                    DBG_MARK(2); DBG_UNIT(3, ord);
+                    mbar_expect_tx(&full[stage], tx_bytes);
+                    if (!amn) tma_load_2d(sA, mA, fbar, kc, ac1);
+                    else { tma_load_2d(sA, mA, fbar, ac0, ac1 + kc); tma_load_2d(sA + 8192u, mA, fbar, ac0 + 64, ac1 + kc); }
+                    if (!bmn) tma_load_2d(sB, mB, fbar, kc, bc1);
+                    else for (int j = 0; j < nB_mn; ++j) tma_load_2d(sB + (uint32_t)j * 8192u, mB, fbar, bc0 + j * 64, kc);
                 }
                 __syncwarp();
-                if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
+                if (++stage == L.stages) { stage = 0; phase ^= 1; }
             }
         }
     } else if (warp == W_PUB0 || warp == W_PUB1) {
         // ================================ publishers ========================================
         // Send every staged 64-column granule of the bf16 outputs to global memory with a TMA store
         // and, once that store has completed (bulk async-group wait: no MEMBAR over the SM's whole store
-        // stream -- a gpu-scope fence issued while epilogue warps stream stores only returns when they
-        // pause), bump the granule's dataflow counter with a release: consumers start on a row block's
+        // stream), bump the granule's dataflow counter with a release: consumers start on a row block's
         // first columns while its last ones are still in the epilogue.  Two publisher threads take the
         // even / odd granules so that one store's completion latency hides behind the other's.
-        // fp32 outputs (dW partials) are stored by the epilogue warps directly and published per unit.
+        // fp32 outputs (dW partials) are stored by the consumer warps directly and published per unit.
+        regs_to_consumers();
         if (lane == 0) {
             const int pub = warp - W_PUB0;
             int acc = 0; uint32_t acc_phase = 0;
@@ -914,99 +840,107 @@ tc_program_kernel(const __grid_constant__ TcLaunch L) {
                         bufs[a] = b; ++sq;
                     }
                     bulk_commit();
-                    if (L.dbg && blockIdx.x == 0 && ord < 24 && g < 4) L.dbg[256 + ord * 8 + 4 + g] = (unsigned long long)clock64();
                     bulk_wait<0>();                          // stores complete: data is in global memory
                     for (int a = 0; a < 2; ++a) if (bufs[a] >= 0) mbar_arrive(&out_free[bufs[a]]);
-                    if (ctr && col0 < ph->N) {
-                        red_release_add(ctr + g, 1);
-                        if (L.dbg && L.n_phases && ord == 0 && g == 0) L.dbg[512 + blockIdx.x] = gtime();
-                        if (L.dbg && L.n_phases && ord == 0 && g == 3) L.dbg[704 + blockIdx.x] = gtime();
-                        if (L.dbg && blockIdx.x == 0 && ord < 24 && g < 4) L.dbg[256 + ord * 8 + g] = (unsigned long long)clock64();
-                    }
+                    if (ctr && col0 < ph->N) red_release_add(ctr + g, 1);
                 }
                 seq += (uint32_t)(gpt * n_arr);
-                mbar_wait(&unit_bar[acc], acc_phase);      // every epilogue warp has finished the unit (direct fp32 stores included)
+                mbar_wait(&unit_bar[acc], acc_phase);      // every consumer warp has finished the unit (direct fp32 stores included)
                 if (ph->done_ctr) red_release_add(ph->done_ctr + u.m_group, 1);
                 if (pub == 1) DBG_UNIT(6, ord);
-                // the barriers of this accumulator stage may be reused: part of the stage's release
-                if (pair && crank == 1) { if constexpr (pair) mbar_arrive_remote(&tempty[acc], 0); } else mbar_arrive(&tempty[acc]);
+                mbar_arrive(&tempty[acc]);                 // the unit barrier of this stage may be reused
                 if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
             }
         }
-    } else {
-        // ================================ epilogue (16 warps) ================================
-        // warp w may read TMEM lanes 32*(w%4)..+31; the four warps of a lane quarter interleave over
-        // the tile's 16-column chunks.
-        const int ew = warp;
-        const int quarter = ew & 3;
+    } else if (warp < CONSUMER_WARPS) {
+        // ================================ consumers (2 warpgroups) ==========================
+        regs_from_producers();
+        const int wg = warp >> 2;
         EpiCtx c;
-        c.sub = ew >> 2; c.lane = lane;
-        c.remote_arrive = pair && crank == 1;
+        c.lane = lane;
         uint32_t out_seq = 0;
         c.seq = &out_seq;
         c.out_base = smem_u32(out_stage); c.out_full = out_full; c.out_free = out_free;
         c.mant_mask = L.mant_mask; c.one_bits = L.one_bits;
-        c.row_off = (uint32_t)(quarter * 32 + lane) * 128u; c.row_swz = (uint32_t)(lane & 7);
-        int acc = 0; uint32_t acc_phase = 0;
+        c.r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        const uint32_t smem_base = smem_u32(smem);
+        const uint32_t wg_off = (uint32_t)wg * 8192u;      // this warpgroup's 64 A rows (either layout)
+        int stage = 0; uint32_t phase = 0;
+        int acc_st = 0; uint32_t acc_phase = 0;
         int pi = 0, ul = -1;
         int ord = -1;
-        const int et = threadIdx.x;                // 0..511: the epilogue threads
+        const int et = threadIdx.x;                // 0..255
+        float acc[NB_MAX][32];
         while (walk_next(pi, ul, cid, n_ops)) {
             ++ord;
             const TcPhaseLite* ph = &c_ph[pi];
             const UnitInfo u = decode_unit(ph, ul);
-            {   // this tile's (pre-scaled) bias slice -> shared memory, while the MMAs are still running
+            // the publishers have finished the unit two back, which used this stage's barrier and bias slice
+            mbar_wait(&tempty[acc_st], acc_phase ^ 1);
+            {   // this tile's (pre-scaled) bias slice -> shared memory
                 const float bsc = (ph->act == ACT_SIGMOID) ? ph->bias_scale * -1.4426950408889634f : ph->bias_scale;
                 const int n = u.n_blk * ph->BN + et;
-                if (et < 256) s_bias[acc * 256 + et] = (ph->bias && et < ph->BN && n < ph->N) ? bsc * __ldg(ph->bias + n) : 0.f;
-                asm volatile("bar.sync 1, 512;" ::: "memory");
-                c.sbias = s_bias + acc * 256;
+                if (et < MAX_BN) s_bias[acc_st * MAX_BN + et] = (ph->bias && et < ph->BN && n < ph->N) ? bsc * __ldg(ph->bias + n) : 0.f;
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+                c.sbias = s_bias + acc_st * MAX_BN;
             }
+            // ---- mainloop: one wgmma group per K chunk, the previous chunk's stage released once its group retired
+            const int bn16 = ph->BN / 16;
+            const int chunks0 = ph->chunks[0];
+            const int cfg0 = (ph->a_mn[0] << 2) | (ph->b_mn[0] << 1) | ph->a_neg[0];
+            const int cfg1 = (ph->a_mn[1] << 2) | (ph->b_mn[1] << 1) | ph->a_neg[1];
+            const bool ordered = ph->dep_chunk_ctr != nullptr;
+            if (threadIdx.x == 0) DBG_UNIT(2, ord);
+            int prev = -1;
+            for (int ci = u.c_begin; ci < u.c_end; ++ci) {
+                const int cc = ordered ? (int)ph->k_order[ci] : ci;     // same order as the producer warp
+                const int cfg = (cc >= chunks0) ? cfg1 : cfg0;
+                const uint32_t sA = smem_base + (uint32_t)stage * (uint32_t)L.stage_bytes;
+                mbar_wait(&full[stage], phase);
+                mma_chunk_any(cfg, bn16, acc, sA + wg_off, sA + (uint32_t)A_BYTES, ci == u.c_begin ? 1u : 0u);
+                wg_wait<1>();
+                if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+                prev = stage;
+                if (++stage == L.stages) { stage = 0; phase ^= 1; }
+            }
+            wg_wait<0>();
+            if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+            if (threadIdx.x == 0) { DBG_MARK(3); DBG_UNIT(3, ord); DBG_UNIT(4, ord); }
+            // ---- epilogue
             c.p.M = ph->M; c.p.N = ph->N; c.p.BN = ph->BN; c.p.act = ph->act; c.p.sample = ph->sample;
             c.p.acc_scale = ph->acc_scale; c.p.bias_scale = ph->bias_scale;
-            c.p.bias = ph->bias; c.p.sigma = ph->sigma; c.p.noise_sigma = ph->noise_sigma;
-            c.p.out_mean_bf = ph->out_mean_bf; c.p.ld_mean_bf = ph->ld_mean_bf;
-            c.p.out_state_bf = ph->out_state_bf; c.p.ld_state_bf = ph->ld_state_bf;
+            c.p.sigma = ph->sigma; c.p.noise_sigma = ph->noise_sigma;
+            c.p.out_mean_bf = ph->out_mean_bf; c.p.out_state_bf = ph->out_state_bf;
             c.p.out_f32 = ph->out_f32; c.p.ld_f32 = ph->ld_f32; c.p.split_stride = ph->split_stride;
             c.p.ais_a = ph->ais_a; c.p.ais_b = ph->ais_b; c.p.ais_next = ph->ais_next; c.p.ais_lin = ph->ais_lin; c.p.ais_logw = ph->ais_logw;
             c.p.ais_ct = ph->ais_b - ph->ais_a; c.p.ais_cd = ph->ais_next - 0.5f * (ph->ais_a + ph->ais_b);
-            const int ph_mode = ph->mode;
             c.rng.k0 = L.k0; c.rng.k1 = L.k1; c.rng.tick = L.tick + ph->tick_off; c.rng.row0 = L.row0; c.rng.c2 = ph->rng_c2;
-            c.m = (u.m_group * CL + crank) * BM + quarter * 32 + lane;
+            c.m0 = (u.m_group * CL + crank) * BM + c.r0;
             c.n_blk = u.n_blk; c.split = u.split;
-            c.tempty = &tempty[acc];
-            mbar_wait_relaxed(&tfull[acc], acc_phase, (uint32_t)L.epi_ns);
-            tc_fence_after();
-            if (threadIdx.x == 0) { DBG_MARK(3); DBG_UNIT(4, ord); }
-            c.t_row = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * ACC_COLS);
-            switch (ph_mode) {
-                case MODE_SIG_BERN_MEAN_STATE: epilogue_tile<MODE_SIG_BERN_MEAN_STATE, pair>(c); break;
-                case MODE_SIG_BERN_STATE: epilogue_tile<MODE_SIG_BERN_STATE, pair>(c); break;
-                case MODE_SIG_MEAN: epilogue_tile<MODE_SIG_MEAN, pair>(c); break;
-                case MODE_RAW_F32: epilogue_tile<MODE_RAW_F32, pair>(c); break;
-                case MODE_AIS_UNITS: epilogue_tile<MODE_AIS_UNITS, pair>(c); break;
-                case MODE_AIS_UNITS_S: epilogue_tile<MODE_AIS_UNITS_S, pair>(c); break;
-                case MODE_AIS_UNITS_G: epilogue_tile<MODE_AIS_UNITS_G, pair>(c); break;
-                case MODE_AIS_STATE: epilogue_tile<MODE_AIS_STATE, pair>(c); break;
-                default: epilogue_tile<MODE_GENERIC, pair>(c); break;
+            switch (ph->mode) {
+                case MODE_SIG_BERN_MEAN_STATE: epilogue_tile<MODE_SIG_BERN_MEAN_STATE>(c, acc); break;
+                case MODE_SIG_BERN_STATE: epilogue_tile<MODE_SIG_BERN_STATE>(c, acc); break;
+                case MODE_SIG_MEAN: epilogue_tile<MODE_SIG_MEAN>(c, acc); break;
+                case MODE_RAW_F32: epilogue_tile<MODE_RAW_F32>(c, acc); break;
+                case MODE_AIS_UNITS: epilogue_tile<MODE_AIS_UNITS>(c, acc); break;
+                case MODE_AIS_UNITS_S: epilogue_tile<MODE_AIS_UNITS_S>(c, acc); break;
+                case MODE_AIS_UNITS_G: epilogue_tile<MODE_AIS_UNITS_G>(c, acc); break;
+                case MODE_AIS_STATE: epilogue_tile<MODE_AIS_STATE>(c, acc); break;
+                default: epilogue_tile<MODE_GENERIC>(c, acc); break;
             }
             if (threadIdx.x == 0) DBG_UNIT(5, ord);
-            // this warp's part of the unit is stored: the publisher warp makes it visible to other SMs
+            // this warp's part of the unit is stored: the publisher warps make it visible to other SMs
             __syncwarp();
-            if (lane == 0) mbar_arrive(&unit_bar[acc]);
+            if (lane == 0) mbar_arrive(&unit_bar[acc_st]);
             if (threadIdx.x == 0) DBG_MARK(4);
-            if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
+            if (++acc_st == ACC_STAGES) { acc_st = 0; acc_phase ^= 1; }
         }
+    } else {
+        regs_to_consumers();         // warp 8: no role
     }
 
-    tc_fence_before();
-    // no CTA may exit while its peer can still signal its barriers or read its shared memory
-    if constexpr (pair) cluster_sync_all(); else __syncthreads();
-    if (warp == W_PUB0) {
-        tc_fence_after();
-        if constexpr (pair) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
-        else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
-    }
+    // no CTA may exit while its bulk stores can still read its shared memory (the publishers waited for them)
+    __syncthreads();
     if (threadIdx.x == 0) { DBG_MARK(5); if (L.dbg && blockIdx.x == 0) L.dbg[7] = gtime(); }
 }
 
@@ -1059,28 +993,25 @@ static CUtensorMap make_map(const TcMat& m, int box0, int box1) {
 
 struct TilePick { int bn, cluster; };
 
-static TilePick pick_tile(int N, bool b_mn, bool staged_out, int m_tiles, int splits, int chunks, int sms, int force_cluster) {
-    // Tile width BN and CTA grouping.  A single SM ingests ~50 B/clk from L2 (measured: the ring of a
-    // 128x256 tile refills at 52 B/clk with one CTA alone on the chip), while tcgen05 at M=128
-    // consumes 8192*(1/128 + 1/BN) B/clk of operands: a lone CTA is ingest-bound.  A CTA pair
-    // (cta_group::2, M=256) halves the B bytes each SM needs.
-    // Cycle model per CTA: waves * chunks * max(mma, ingest) + epilogue of the last tile.
-    TilePick best{b_mn ? 64 : 16, 1};
+static TilePick pick_tile(int N, int m_tiles, int splits, int chunks, int sms, int force_cluster) {
+    // Tile width BN (64 or 128: whole 64-column wgmma blocks and TMA-store granules) and row grouping (CTAs
+    // taking one 128-row block each, or pairs taking a 256-row group).  Cycle model per CTA:
+    // waves * chunks * max(mma, ingest) + epilogue of the last tile, with the tensor cores at ~2048 bf16
+    // MACs/clk per SM (989 TFLOP/s dense over 132 SMs) and L2 ingest assumed at ~32 B/clk per SM (not measured).
+    TilePick best{64, 1};
     double best_cost = 1e30;
     for (int c = 1; c <= 2; ++c) {
         if (force_cluster && c != force_cluster) continue;
         if (!force_cluster && c == 2 && m_tiles < 2) break;
-        // every CTA of a pair holds BN/2 columns of B (whole boxes / 8-row atoms); bf16 outputs leave in
-        // 64-column TMA-store granules, so their tiles are whole granules wide (the tensor edge clips)
-        const int step = b_mn ? 64 * c : (staged_out ? 64 : 16);
-        const int slots = sms / c;
-        for (int bn = step; bn <= 256; bn += step) {
+        const int slots = sms / c * c;                 // CTAs of the grid
+        // (192 / 256 and widths of 16-column steps are reachable through force_bn only: a 256-wide tile leaves 3 ring stages)
+        for (int bn = 64; bn <= 128; bn += 64) {
             const int nt = (N + bn - 1) / bn;
             const int m_groups = (m_tiles + c - 1) / c;
-            const long units = (long)m_groups * nt * splits;
+            const long units = (long)m_groups * c * nt * splits;
             const long waves = (units + slots - 1) / slots;
-            const double mma = 4.0 * (bn / 2.0);                                  // cycles per K chunk (4 x K=16)
-            const double ingest = (16384.0 + (bn / c) * 128.0) / 45.0;           // bytes per chunk per SM / (B/clk)
+            const double mma = (double)BM * bn * BK / 2048.0;                     // cycles per K chunk
+            const double ingest = (double)(A_BYTES + bn * BK * 2) / 32.0;         // bytes per chunk per SM / (B/clk)
             const double cost = (double)waves * chunks * (mma > ingest ? mma : ingest) + 12.0 * bn;
             if (cost < best_cost - 1e-9) { best_cost = cost; best.bn = bn; best.cluster = c; }
         }
@@ -1114,17 +1045,17 @@ static void fill_phase(Ctx* ctx, const TcGemm& g, int cluster, TcPhase& ph) {
     memset(&ph, 0, sizeof(ph));
     p.M = g.M; p.N = g.N; p.n_pairs = g.n_pairs;
     const int m_tiles = (g.M + BM - 1) / BM;
-    bool need64 = false;
-    for (int i = 0; i < g.n_pairs; ++i) need64 = need64 || g.b_t[i];
     int chunks_total = 0;
     for (int i = 0; i < g.n_pairs; ++i) chunks_total += (g.K[i] + BK - 1) / BK;
     const int nsplit = g.splits > 0 ? g.splits : 1;
-    const bool staged_out = g.out_mean_bf != nullptr || g.out_state_bf != nullptr;
-    TilePick tp = pick_tile(g.N, need64, staged_out, m_tiles, nsplit, (chunks_total + nsplit - 1) / nsplit, ctx->sm_count, cluster);
+    TilePick tp = pick_tile(g.N, m_tiles, nsplit, (chunks_total + nsplit - 1) / nsplit, ctx->sm_count, cluster);
     if (g.force_bn > 0) tp.bn = g.force_bn;
-    BM_REQUIRE(tp.cluster == cluster, "tile picker returned another cluster size");
-    BM_REQUIRE(cluster == 1 || (need64 ? tp.bn % 128 == 0 : tp.bn % 16 == 0), "CTA-pair tiles need BN/2 on whole boxes / swizzle atoms");
-    BM_REQUIRE(tp.bn % 16 == 0 && tp.bn <= 256 && (!need64 || tp.bn % 64 == 0), "bad tile width");
+    BM_REQUIRE(tp.cluster == cluster, "tile picker returned another row grouping");
+    bool b_mn = false;
+    for (int i = 0; i < g.n_pairs; ++i) b_mn = b_mn || g.b_t[i];
+    const bool staged_out = g.out_mean_bf != nullptr || g.out_state_bf != nullptr;
+    BM_REQUIRE(tp.bn % 16 == 0 && tp.bn >= 16 && tp.bn <= MAX_BN, "tile width must be a multiple of 16 columns, at most 256");
+    BM_REQUIRE(!b_mn || tp.bn % 64 == 0, "an MN-major B operand needs tiles of whole 64-column boxes");
     BM_REQUIRE(!staged_out || tp.bn % 64 == 0, "ops with bf16 outputs need tiles of whole 64-column granules");
     p.BN = tp.bn;
     p.gran_per_tile = (p.BN + GRAN_COLS - 1) / GRAN_COLS;
@@ -1137,9 +1068,9 @@ static void fill_phase(Ctx* ctx, const TcGemm& g, int cluster, TcPhase& ph) {
         p.chunks[i] = i < g.n_pairs ? (g.K[j] + BK - 1) / BK : 0;
         p.a_mn[i] = g.a_t[j]; p.b_mn[i] = g.b_t[j]; p.a_neg[i] = g.neg[j];
         p.a_row0[i] = g.a_row0[j]; p.a_k0[i] = g.a_k0[j]; p.a_batch[i] = g.a_batch[j];
-        // K-major: box = 64 k x (128 | BN/cluster) rows; MN-major: box = 64 mn x 64 k
+        // K-major: box = 64 k x (128 | BN) rows; MN-major: box = 64 mn x 64 k
         ph.tmA[i] = g.a_t[j] ? make_map(g.A[j], 64, 64) : make_map(g.A[j], 64, BM);
-        ph.tmB[i] = g.b_t[j] ? make_map(g.B[j], 64, 64) : make_map(g.B[j], 64, p.BN / cluster);
+        ph.tmB[i] = g.b_t[j] ? make_map(g.B[j], 64, 64) : make_map(g.B[j], 64, p.BN);
         BM_REQUIRE(i >= g.n_pairs || g.K[j] > 0, "tensor-core GEMM pair with K == 0");
     }
     BM_REQUIRE(p.splits <= chunks_total, "more K splits than K chunks");
@@ -1196,19 +1127,22 @@ static void do_launch(Ctx* ctx, TcLaunch& L, int cluster, double flops, int max_
         attr_set[ctx->device & 63] = true;
     }
     // ring stages sized for the widest tile of the launch: narrower tiles buy a deeper pipeline
-    L.stage_bytes = A_BYTES + (max_bn / cluster) * BK * 2;
+    L.stage_bytes = A_BYTES + max_bn * BK * 2;
     L.stage_bytes = (L.stage_bytes + 1023) & ~1023;           // 128B-swizzle atoms are 1024-byte aligned
     L.stages = RING_BYTES / L.stage_bytes;
     if (L.stages > MAX_STAGES) L.stages = MAX_STAGES;
     { const char* e = getenv("BM_TC_STAGES"); if (e && atoi(e) >= 2 && atoi(e) <= L.stages) L.stages = atoi(e); }
-    const int max_clusters = ctx->sm_count / cluster;
+    const int max_groups = ctx->sm_count / cluster;
     // programs address pairs by number (TcPhaseLite::pair_begin/pair_count): launch all of them
-    const int n_clusters = L.n_phases ? max_clusters : (L.total_units < max_clusters ? L.total_units : max_clusters);
+    const int n_groups = L.n_phases ? max_groups : (L.total_units < max_groups ? L.total_units : max_groups);
+    const int n_ctas = n_groups * cluster;
+    // The CTAs of a pair share nothing, so the grid is launched as clusters of one CTA: a pair never has to fit into
+    // one GPC, and the residency question below counts single CTAs.
     cudaLaunchConfig_t lc{};
-    lc.gridDim = dim3(n_clusters * cluster); lc.blockDim = dim3(TC_THREADS); lc.dynamicSmemBytes = SMEM_BYTES; lc.stream = ctx->stream;
+    lc.gridDim = dim3(n_ctas); lc.blockDim = dim3(TC_THREADS); lc.dynamicSmemBytes = SMEM_BYTES; lc.stream = ctx->stream;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    at[0].val.clusterDim.x = 1; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
     lc.attrs = at; lc.numAttrs = 1;
     if (L.n_phases) {
         // a program's CTAs wait for each other through counters in global memory: all of them must be resident at once.  Ask the
@@ -1223,14 +1157,13 @@ static void do_launch(Ctx* ctx, TcLaunch& L, int cluster, double flops, int max_
             else if (cudaOccupancyMaxActiveClusters(&n, cluster == 2 ? (const void*)tc_program_kernel<2> : (const void*)tc_program_kernel<1>, &lc) == cudaSuccess) r = n > 0 ? n : -2;
             else { cudaGetLastError(); r = -1; }
             if (getenv("BM_TC_DEBUG_RESIDENCY"))
-                fprintf(stderr, "[bm] device %d: cudaOccupancyMaxActiveClusters(tc_program_kernel<%d>) = %d, the program grid has %d clusters\n",
-                        ctx->device, cluster, n, n_clusters);
+                fprintf(stderr, "[bm] device %d: cudaOccupancyMaxActiveClusters(tc_program_kernel<%d>) = %d, the program grid has %d CTAs\n",
+                        ctx->device, cluster, n, n_ctas);
         }
-        BM_REQUIRE(r == -1 || r >= n_clusters,
+        BM_REQUIRE(r == -1 || r >= n_ctas,
                    "the device cannot hold all CTA clusters of a dataflow program at once (cudaOccupancyMaxActiveClusters); it would deadlock");
     }
     if (ctx->profile_tc) BM_CUDA(cudaEventRecord(profile_event(ctx), ctx->stream));
-    // kernels that contain cta_group::2 instructions must be launched as clusters of 2: separate instantiations
     if (cluster == 2) BM_CUDA(cudaLaunchKernelEx(&lc, tc_program_kernel<2>, L));
     else BM_CUDA(cudaLaunchKernelEx(&lc, tc_program_kernel<1>, L));
     if (ctx->profile_tc) {
@@ -1251,11 +1184,6 @@ void launch_tc_gemm(Ctx* ctx, const TcGemm& g) {
     const int m_tiles = (g.M + BM - 1) / BM;
     int cluster = g.force_cluster > 0 ? g.force_cluster : (m_tiles >= 2 ? 2 : 1);
     BM_REQUIRE(cluster == 1 || cluster == 2, "cluster must be 1 or 2");
-    if (cluster == 2) {      // fall back to single CTAs when the B tile cannot be halved on box boundaries
-        bool need64 = false;
-        for (int i = 0; i < g.n_pairs; ++i) need64 = need64 || g.b_t[i];
-        if (need64 && g.N < 128 && !g.force_cluster) cluster = 1;
-    }
     TcLaunch L;
     memset(&L, 0, sizeof(L));
     fill_phase(ctx, g, cluster, L.inl);
@@ -1436,22 +1364,10 @@ void launch_tc_program(Ctx* ctx, TcProgram& prog, RngKey rng, int batch_row) {
                 h[1] - h[0], h[5] - h[0], h[7] - h[6], unit);
         fprintf(stderr, "  unit 1 tma_issue:");
         for (int i = 0; i < 24 && h[8 + i]; ++i) fprintf(stderr, " %llu", h[8 + i] - h[0]);
-        fprintf(stderr, "\n  first-unit granule 0 / granule 3 publish time per CTA (ns after CTA 0 start):");
-        for (int i = 0; i < 148; ++i) if (h[512 + i]) fprintf(stderr, " %d:%lld/%lld", i, (long long)(h[512 + i] - h[6]), (long long)(h[704 + i] - h[6]));
-        fprintf(stderr, "\n  unit 1 poll ok (time:upto):");
-        for (int i = 0; i < 20; ++i) if (h[456 + i]) fprintf(stderr, " [%d] %llu:%llu", i, h[456 + i] - h[0], h[480 + i]);
-        fprintf(stderr, "\n  unit 1 fenced:");
-        for (int i = 0; i < 20; ++i) if (h[432 + i]) fprintf(stderr, " [%d] %llu", i, h[432 + i] - h[0]);
-        fprintf(stderr, "\n  unit 1 mma_ready:");
-        for (int i = 0; i < 24 && h[32 + i]; ++i) fprintf(stderr, " %llu", h[32 + i] - h[0]);
         fprintf(stderr, "\n  ord: start dep_ok mma_first mma_done epi_start epi_done published\n");
         for (int o = 0; o < 24 && h[64 + o * 8]; ++o) {
             fprintf(stderr, "  %2d:", o);
             for (int k = 0; k < 7; ++k) fprintf(stderr, " %7llu", h[64 + o * 8 + k] ? h[64 + o * 8 + k] - h[0] : 0ull);
-            fprintf(stderr, "   | granule staged:");
-            for (int k = 4; k < 8; ++k) fprintf(stderr, " %7llu", h[256 + o * 8 + k] ? h[256 + o * 8 + k] - h[0] : 0ull);
-            fprintf(stderr, " published:");
-            for (int k = 0; k < 4; ++k) fprintf(stderr, " %7llu", h[256 + o * 8 + k] ? h[256 + o * 8 + k] - h[0] : 0ull);
             fprintf(stderr, "\n");
         }
     }

@@ -1,4 +1,4 @@
-// Tensor-core (tcgen05 / TMEM / TMA) path of libbm.so: host-side description of fused
+// Tensor-core (wgmma / TMA) path of libbm.so: host-side description of fused
 // "layer ops" and of multi-phase programs (a whole Gibbs chain + dW in ONE persistent launch).
 // Kernel in bm_tc.cu.
 #pragma once
@@ -15,7 +15,7 @@ struct TcMat {
     int rows = 0, cols = 0, ld = 0;
 };
 
-// C[M,N] (fp32, TMEM) = sum over pairs of  (+/-) A_p[M,K_p] * B_p[N,K_p]^T
+// C[M,N] (fp32, registers) = sum over pairs of  (+/-) A_p[M,K_p] * B_p[N,K_p]^T
 //   a_t == false: A_p is stored [M, K] (K contiguous, "K-major");  true: stored [K, M] (M contiguous, "MN-major")
 //   b_t == false: B_p is stored [N, K] (K-major);                 true: stored [K, N] (MN-major)
 // then the same fused epilogue as the CUDA-core LayerOp (bias, scale, activation, Philox sampling),
@@ -25,13 +25,13 @@ struct TcGemm {
     int n_pairs = 1;
     TcMat A[2], B[2];
     bool a_t[2] = {false, false}, b_t[2] = {false, false};
-    bool neg[2] = {false, false};     // subtract this pair (tcgen05 a_negate)
+    bool neg[2] = {false, false};     // subtract this pair (wgmma scale-a = -1)
     int K[2] = {0, 0};
     int a_row0[2] = {0, 0};           // first row of A_p inside its buffer (resident dataset slices; !a_t only)
     int a_k0[2] = {0, 0};             // first K row of A_p inside its buffer (a_t only)
     bool a_batch[2] = {false, false}; // add the launch's batch_row to a_row0 / a_k0 (resident dataset cursor)
     unsigned long long* dbg = nullptr;     // device buffer of 64 timestamps (debug timeline)
-    int force_bn = 0, force_cluster = 0;   // tests: override the tile heuristic
+    int force_bn = 0, force_cluster = 0;   // tests: override the tile heuristic (width; CTA pairs or single CTAs)
     // split-K: the concatenated K range is cut into `splits` parts; part s writes out_f32 + s * split_stride
     int splits = 1;
     size_t split_stride = 0;

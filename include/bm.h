@@ -1,4 +1,4 @@
-/* bm.h -- C-ABI of libbm.so: the B200-native RBM/DBM engine.
+/* bm.h -- C-ABI of libbm.so: the H100-native RBM/DBM engine.
  *
  * This is the drop-in boundary.  In the reference (yell/boltzmann-machines) the
  * operator boundary of the hot path is "a TensorFlow graph with named
@@ -28,7 +28,7 @@ extern "C" {
 #define BM_OK            0
 #define BM_EINVAL       -1   /* bad argument / shape / name                     */
 #define BM_ECUDA        -2   /* CUDA runtime or driver error                    */
-#define BM_ENOGPU       -3   /* no usable sm_100 device                         */
+#define BM_ENOGPU       -3   /* no usable sm_90 device                          */
 #define BM_ENCCL        -4   /* NCCL missing or failed                          */
 #define BM_EUNSUPPORTED -5   /* configuration not implemented by the engine     */
 
@@ -39,7 +39,7 @@ typedef struct bm_dbm bm_dbm;   /* one DBM: layers, variational params, particle
 enum { BM_UNIT_BERNOULLI = 0, BM_UNIT_MULTINOMIAL = 1, BM_UNIT_GAUSSIAN = 2 };  /* layers.py:39-89 */
 enum { BM_DTYPE_F32 = 0, BM_DTYPE_F64 = 1 };                                     /* base/mixin.py:14-25 */
 enum { BM_COMPUTE_FP32 = 0,   /* CUDA-core FMA, storage dtype everywhere (parity anchor) */
-       BM_COMPUTE_BF16 = 1 }; /* tcgen05 bf16 operands, fp32 accumulate (F32 models only) */
+       BM_COMPUTE_BF16 = 1 }; /* wgmma bf16 operands, fp32 accumulate (F32 models only)   */
 
 /* metric selection bits / slots of the double[4] result (base_rbm.py:482-517) */
 enum { BM_METRIC_L2_LOSS = 1, BM_METRIC_MSRE = 2, BM_METRIC_PLL = 4, BM_METRIC_FREE_ENERGY = 8 };

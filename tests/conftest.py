@@ -32,7 +32,7 @@ def _build_if_missing():
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100)')
     if not hasattr(config, 'workerinput'):            # (pytest-xdist: only the controller builds)
         _build_if_missing()
     if os.environ.get('BM_HOSTSIM') == '1':
@@ -53,9 +53,9 @@ def pytest_configure(config):
         config._bm_hostsim = lib
 
 
-# GPU tests written after the last visit to a B200 (they pass on the host simulation, tests/hostsim): run them after the tests that
+# GPU tests not yet run on an H100 (they pass on the host simulation, tests/hostsim): run them after the tests that
 # have already passed on the hardware, so that `-x` reports a surprise in one of them without hiding the rest of the suite.
-NOT_YET_RUN_ON_A_B200 = ()       # (round 2, visits q / r: every GPU test has passed on the hardware)
+NOT_YET_RUN_ON_A_GPU = ()
 
 
 def pytest_collection_modifyitems(config, items):
@@ -67,7 +67,7 @@ def pytest_collection_modifyitems(config, items):
         ids = set(id(it) for it in void)
         items[:] = [it for it in items if id(it) not in ids]
         config.hook.pytest_deselected(items=void)
-    late = [it for it in items if it.get_closest_marker('gpu') and any(tag in it.nodeid for tag in NOT_YET_RUN_ON_A_B200)]
+    late = [it for it in items if it.get_closest_marker('gpu') and any(tag in it.nodeid for tag in NOT_YET_RUN_ON_A_GPU)]
     if late:
         ids = set(id(it) for it in late)
         items[:] = [it for it in items if id(it) not in ids] + late

@@ -137,7 +137,10 @@ def _stub_modules(n_train, n_test):
 
 
 def run_example(path, argv, n_train=640, n_test=128):
-    """Executes the example at `path` as __main__ with command line `argv`.  Returns the script's globals."""
+    """Executes the example at `path` as __main__ with command line `argv`.  Returns the script's globals.
+
+    No test calls it: the examples are the reference project's source and are not stored here.  It is kept for running them by
+    hand against a checkout of the reference, e.g. `run_example('<checkout>/examples/rbm_mnist.py', ['--n-train', '512'])`."""
     src = open(path).read()
     py3 = translate(src)
     code = compile(py3, path, 'exec')

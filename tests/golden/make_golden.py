@@ -1,6 +1,6 @@
 """Generates tests/golden/reference_utils.json by IMPORTING the reference's own modules.
 
-Run in the build container only (it reads /root/reference, which does not exist on the GPU box):
+Needs a checkout of yell/boltzmann-machines, named by the BM_REFERENCE_DIR environment variable:
 
     python tests/golden/make_golden.py
 
@@ -16,7 +16,7 @@ import os
 
 import numpy as np
 
-REF = '/root/reference/boltzmann_machines/utils'
+REF = os.path.join(os.environ['BM_REFERENCE_DIR'], 'boltzmann_machines', 'utils')
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 

@@ -1,11 +1,11 @@
 """Golden vectors from the REFERENCE'S OWN RBM AND DBM CODE: tests/golden/reference_rbm_cases.json,
 tests/golden/reference_dbm_cases.json.
 
-Run in the build container only (reads /root/reference):
+Needs a checkout of yell/boltzmann-machines, named by the BM_REFERENCE_DIR environment variable:
 
     python tests/golden/make_reference_golden.py
 
-yell/boltzmann-machines is imported unmodified from /root/reference with `oracle/tf1shim.py` registered as
+yell/boltzmann-machines is imported unmodified from that checkout with `oracle/tf1shim.py` registered as
 `tensorflow` (TensorFlow 1.3 itself cannot be installed here).  For every case below the reference's own
 `BernoulliRBM/GaussianRBM/MultinomialRBM(...).fit(X, X_val)`, `.transform(X)`, `.get_tf_params(...)` and `.init()` run:
 its graph construction (base_rbm.py:244-525), its fit loop (:533-655), its persistence round trip between public calls
@@ -526,7 +526,8 @@ def main():
     args = ap.parse_args()
     tf1shim.default_random_provider = provider
     tf1shim.install()
-    sys.path[:0] = ['/root/reference', '/root/reference/boltzmann_machines']
+    REF_DIR = os.path.abspath(os.environ['BM_REFERENCE_DIR'])
+    sys.path[:0] = [REF_DIR, os.path.join(REF_DIR, 'boltzmann_machines')]
     # rbm/rbm.py imports `layers` as a top-level module (rbm/env.py puts the package directory on sys.path) while dbm.py
     # imports `.layers`: two module objects, and DBM.log_Z / log_proba assert isinstance(layer, BernoulliLayer) across
     # them (dbm.py:927,948).  Serve the one module under both names -- an import alias, no source change.
@@ -546,7 +547,7 @@ def main():
             pass
     sys.meta_path.insert(0, _LayersAlias())
     import boltzmann_machines as ref                     # the reference package, unmodified
-    assert ref.__file__.startswith('/root/reference/'), ref.__file__
+    assert ref.__file__.startswith(REF_DIR + os.sep), ref.__file__
     if not args.fuzz:
         write_layer_goldens(ref)
     work = tempfile.mkdtemp(prefix='bm_golden_')

@@ -1,5 +1,5 @@
 #!/bin/bash
-# TEST INFRASTRUCTURE: links libbm's own objects (built by ../../build.sh for sm_100a) against tests/hostsim/fake_cudart.cpp
+# TEST INFRASTRUCTURE: links libbm's own objects (built by ../../build.sh for sm_90a) against tests/hostsim/fake_cudart.cpp
 # instead of libcudart -> tests/hostsim/_build/libbm_hostsim.so: the host side of the library runs without a GPU
 # (kernel launches are recorded and skipped; see fake_cudart.cpp for what is checked).
 # Safe to call from several processes at once (pytest-xdist workers): one builds under a lock, outputs appear by rename, and nothing

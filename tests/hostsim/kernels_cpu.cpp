@@ -34,7 +34,7 @@ bool dropped_dependency(int op, int d);
 
 // what fake_encode_tiled stores in the opaque CUtensorMap
 struct MapView { const void* base; unsigned long long cols, rows, ld_bytes; unsigned box0, box1; unsigned magic; };
-static const unsigned MAP_MAGIC = 0xB200C0DEu;
+static const unsigned MAP_MAGIC = 0x590AC0DEu;
 
 static inline float bf2f(__nv_bfloat16 v) { unsigned short b; memcpy(&b, &v, 2); unsigned u = (unsigned)b << 16; float f; memcpy(&f, &u, 4); return f; }
 static inline __nv_bfloat16 f2bf(float f) {           // round to nearest even, as __float2bfloat16_rn
@@ -249,7 +249,7 @@ static void run_tc_op(const bm::TcPhase& ph, const bm::TcLaunch& L, Hazards* hz 
                     if (p.out_state_bf) p.out_state_bf[(size_t)m * p.ld_state_bf + n] = f2bf(state);
                     if (p.out_f32) (p.out_f32 + (size_t)split * p.split_stride)[(size_t)m * p.ld_f32 + n] = mean;
                     if (n == p.N - 1 && (p.N & 7) != 0) {
-                        // Observed on the B200 (round 2): a TMA store box clipped by the tensor edge INSIDE a 16-byte unit leaves
+                        // Observed on the hardware: a TMA store box clipped by the tensor edge INSIDE a 16-byte unit leaves
                         // the rest of that unit overwritten.  Modelled as poison, so that nothing may keep data there.
                         const int end = (p.N + 7) & ~7;
                         for (int c = p.N; c < end; ++c) {

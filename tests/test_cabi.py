@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol():
     lib = _native.load_library()
     for name in declared_symbols():
         assert hasattr(lib, name), name
-    assert b'sm_100a' in lib.bm_version()
+    assert b'sm_90a' in lib.bm_version()
 
 
 def test_no_cpu_fallback_without_gpu():

@@ -2,7 +2,7 @@
 (tests/hostsim/fake_cudart.cpp: device memory is host memory, kernel launches are recorded and skipped).
 
 Every entry point of the RBM and DBM engines -- including the tensor-core DBM engine and its persistent-program variants,
-which have not run on a B200 yet -- is driven through the C-ABI on benchmark-sized and ragged shapes.  What this checks:
+which have not run on a GPU yet -- is driven through the C-ABI on benchmark-sized and ragged shapes.  What this checks:
 every BM_REQUIRE on the way, every tensor map the host encodes (validated like the driver does, and its whole view must
 lie inside one device allocation), every memcpy / memset range against the allocation it touches, launch configurations,
 program construction (dependencies, op counts).  What it cannot check: anything a kernel computes."""
@@ -570,7 +570,7 @@ def test_program_dataflow_hazards_are_checked_and_a_missing_dependency_is_caught
 def test_gpu_tests_of_round_two_features_pass_on_the_interpreter(selection):
     """The GPU tests written in round 2 -- user-defined layers on the plugin engine, multinomial layers on the tensor-core path,
     chains cut into several program launches, the packed feeds -- dry-run here through the library's own host code with interpreted
-    kernels (BM_HOSTSIM=1, see conftest.py): their host side is covered by the CPU suite, their kernels by the B200 runs."""
+    kernels (BM_HOSTSIM=1, see conftest.py): their host side is covered by the CPU suite, their kernels by the GPU runs."""
     import subprocess
     import sys
     env = dict(os.environ, BM_HOSTSIM='1')

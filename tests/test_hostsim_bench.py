@@ -18,7 +18,7 @@ from boltzmann_machines import _native
 sim = _native.load_library({sim!r})
 sim.fakecuda_violation.restype = C.c_char_p
 _native._lib = sim
-sys.argv = ['bench.py', '--steps', '6', '--warmup', '3', '--no-cpu-baseline']
+sys.argv = ['bench.py', '--steps', '6', '--warmup', '3', '--no-cpu-baseline', '--dump-outputs', 'dump']
 try:
     runpy.run_path({bench!r}, run_name='__main__')
 finally:
@@ -51,10 +51,40 @@ def test_bench_contract_on_the_host_simulation(tmp_path):
     assert out['e2e']['h2d_bytes_per_step'] == 4096 * 784          # one byte per visible unit and row
     assert 'fit_region_failed' not in out['e2e'] and out['e2e']['path'].startswith('Model(**kwargs).fit(X)')
     assert out['gpu_launches'] == 2 * out['steps']                  # the step's program and the update kernel
+    # --dump-outputs: the model the last timed step left behind, float32, under the cap
+    import numpy as np
+    dump = tmp_path / 'dump'
+    got = {f.name: np.load(str(f)) for f in dump.iterdir()}
+    assert set(got) == {'W.npy', 'vb.npy', 'hb.npy'}, sorted(got)
+    assert got['W.npy'].shape == (784, 1024) and got['vb.npy'].shape == (784,) and got['hb.npy'].shape == (1024,)
+    assert all(a.dtype == np.float32 for a in got.values())
+
+
+def test_dump_outputs_samples_what_exceeds_the_cap(tmp_path, monkeypatch):
+    """bench.dump_outputs: float64 stays float64, other arrays become float32; an array that would take the total past the cap
+    is replaced by a fixed, seeded sample of its elements plus their indices, and the same input gives the same files."""
+    import importlib.util
+    import numpy as np
+    # a private copy of the module: other tests import `bench` with their own environment
+    spec = importlib.util.spec_from_file_location('bench_under_test', os.path.join(ROOT, 'bench.py'))
+    bench = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(bench)
+    monkeypatch.setattr(bench, 'DUMP_BYTES', 4000)
+    arrays = {'small': np.arange(10, dtype=np.float64), 'big': np.arange(5000, dtype=np.int32).reshape(50, 100)}
+    for d in ('a', 'b'):
+        bench.dump_outputs(str(tmp_path / d), arrays)
+    small, big, idx = (np.load(str(tmp_path / 'a' / n)) for n in ('small.npy', 'big.npy', 'big_index.npy'))
+    assert small.dtype == np.float64 and np.array_equal(small, arrays['small'])
+    assert big.dtype == np.float32 and np.array_equal(big, arrays['big'].reshape(-1)[idx].astype(np.float32))
+    assert np.all(np.diff(idx) > 0) and 0 < big.size < 5000
+    total = sum(f.stat().st_size for f in (tmp_path / 'a').iterdir())
+    assert total <= 4000 + 3 * 128                                      # (+ the .npy headers)
+    for n in ('small.npy', 'big.npy', 'big_index.npy'):
+        assert np.array_equal(np.load(str(tmp_path / 'a' / n)), np.load(str(tmp_path / 'b' / n)))
 
 
 def test_reference_arm_prints_the_same_config_and_runs_exactly_the_steps_it_was_given(tmp_path):
-    """`bench.py --impl reference --steps K --warmup W`: the oracle port on the host cores; same `config` object as the b200 arm,
+    """`bench.py --impl reference --steps K --warmup W`: the oracle port on the host cores; same `config` object as the CUDA arm,
     exactly K timed steps (each a bounded sample of the workload's step when K full steps would not fit the time budget), and the
     cpu_baseline / e2e objects the contract asks of this arm."""
     env = dict(os.environ, BM_BENCH_REFERENCE_SECONDS='3', BM_BENCH_BATCHES='20')

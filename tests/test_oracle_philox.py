@@ -1,5 +1,5 @@
 """Pins the oracle's RNG against the reference's own known-answer test
-(/root/reference/boltzmann_machines/rbm/tests/test_rbm.py:52-67)."""
+(the reference's boltzmann_machines/rbm/tests/test_rbm.py:52-67)."""
 import numpy as np
 from numpy.testing import assert_almost_equal
 

@@ -1,5 +1,5 @@
 """Port of the reference's RBM tests
-(/root/reference/boltzmann_machines/rbm/tests/test_rbm.py) exercising the
+(the reference's boltzmann_machines/rbm/tests/test_rbm.py) exercising the
 package's host logic -- schedules, save/load, resume, determinism -- with the
 numpy oracle plugged in as the engine (CPU, `-m "not gpu"`), and with the CUDA
 engine in both compute modes (`-m gpu`): the `engines` fixture is parametrised."""

@@ -1,4 +1,4 @@
-"""Tensor-core (tcgen05) path: the raw GEMM in every operand layout, then the bf16 RBM engine
+"""Tensor-core (wgmma) path: the raw GEMM in every operand layout, then the bf16 RBM engine
 against the oracle that rounds at the same points (bf16 operands, fp32 accumulation)."""
 import numpy as np
 import pytest
@@ -36,10 +36,11 @@ def test_raw_gemm_all_layouts(M, N, K, a_t, b_t):
 @pytest.mark.parametrize('a_t', [False, True])
 @pytest.mark.parametrize('b_t', [False, True])
 def test_cta_pair_tiles(cluster, bn, a_t, b_t):
-    """cta_group::2: a CTA pair computes a 256-row tile, each CTA holding half of the B tile;
-    ragged row-block pairs (M = 5 tiles -> the last pair has an empty peer), many K chunks."""
-    if b_t and bn % (64 * cluster):
-        pytest.skip('MN-major B: every CTA holds whole 64-column boxes')
+    """Forced tile widths (whole 64-column wgmma blocks plus a last block of 16 / 32 / 48 columns), with CTA pairs taking
+    256-row groups or single CTAs taking 128-row blocks; ragged row-block pairs (M = 5 tiles -> the last pair has an empty
+    peer), ragged column tiles, many K chunks."""
+    if b_t and bn % 64:
+        pytest.skip('MN-major B: a tile holds whole 64-column boxes')
     rng = np.random.RandomState(cluster * 1000 + bn)
     M, N, K = 600, 784, 840
     A = rng.randn(K, M) if a_t else rng.randn(M, K)
@@ -187,7 +188,7 @@ def test_bf16_training_tracks_fp32_statistically():
 @pytest.mark.parametrize('kind', ['multinomial', 'multinomial-v'])
 @pytest.mark.parametrize('V,H,B,k', [(130, 70, 65, 1), (784, 256, 128, 2), (37, 29, 19, 3)])
 def test_multinomial_layers_on_the_tensor_cores_match_the_rounding_oracle(kind, V, H, B, k):
-    """layers.py:54-70 with the GEMMs on tcgen05 (raw fp32 pre-activations -> row softmax -> categorical draws on the unrounded
+    """layers.py:54-70 with the GEMMs on the tensor cores (raw fp32 pre-activations -> row softmax -> categorical draws on the unrounded
     means -> bf16 operands of the next GEMM), against the oracle that rounds at the same points: activations to a bf16 ulp,
     counts from the shared Philox stream, the whole update."""
     cfg = make_cfg(kind, V, H, B)

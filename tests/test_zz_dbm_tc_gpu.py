@@ -1,8 +1,8 @@
 """Tensor-core DBM engine (compute='bf16', csrc/bm_dbm_tc.cuh) against its bf16-operand emulation
 (oracle/dbm_bf16.py), the pinned fp32 oracle and exact enumeration.
 
-First run on a B200 in round 2 (`profiles/r02_a_*`): all green, both operand-layout variants; the engine is the default for
-float32 models with Bernoulli hidden layers since."""
+Both operand-layout variants; the engine is the default for
+float32 models with Bernoulli hidden layers."""
 import os
 
 import numpy as np

@@ -3,8 +3,7 @@
 The fixed-shape parity tests pin a handful of tile geometries; this one walks ragged sizes (visible / hidden / batch
 counts that are not multiples of 8, 64 or 128, single-row batches, K shorter than one MMA chunk), every unit kind,
 dropout, sampling flags and chain lengths through `bm_rbm_train_step` / `bm_dbm_train_step` in each compute mode.
-
-First run on a B200 in round 2: 100 of 100 cases green."""
+"""
 import os
 
 import numpy as np
