@@ -27,7 +27,7 @@ EXPORTS = (
     'bm_ctx_launch_count', 'bm_ctx_profile_tc', 'bm_ctx_profile_read', 'bm_comm_unique_id', 'bm_ctx_comm_init',
     'bm_rbm_create', 'bm_rbm_destroy', 'bm_rbm_set_param', 'bm_rbm_get_param', 'bm_rbm_init_weights',
     'bm_rbm_train_step', 'bm_rbm_set_data', 'bm_rbm_train_step_at', 'bm_rbm_train_epoch', 'bm_rbm_train_epoch_u8', 'bm_rbm_train_epoch_bf16', 'bm_rbm_transform', 'bm_rbm_metrics',
-    'bm_rbm_get_activation', 'bm_debug_tc_gemm',
+    'bm_rbm_get_activation', 'bm_debug_tc_gemm', 'bm_debug_tc_op',
     'bm_dbm_create', 'bm_dbm_destroy', 'bm_dbm_set_param', 'bm_dbm_get_param', 'bm_dbm_init_particles',
     'bm_dbm_train_step', 'bm_dbm_val_metrics', 'bm_dbm_transform', 'bm_dbm_reconstruct', 'bm_dbm_log_proba',
     'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows',
@@ -64,6 +64,27 @@ class DbmCfg(C.Structure):
         ('sparsity_target', C.POINTER(C.c_double)),
         ('sparsity_cost', C.POINTER(C.c_double)),
         ('sigma', C.POINTER(C.c_double)),
+    ]
+
+
+class TcOpArgs(C.Structure):
+    _fields_ = [
+        ('M', C.c_int32), ('N', C.c_int32), ('n_pairs', C.c_int32),
+        ('K', C.c_int32 * 2), ('a_t', C.c_int32 * 2), ('b_t', C.c_int32 * 2), ('neg', C.c_int32 * 2),
+        ('A', C.c_void_p * 2), ('B', C.c_void_p * 2),
+        ('splits', C.c_int32), ('force_bn', C.c_int32), ('force_cluster', C.c_int32),
+        ('acc_scale', C.c_float), ('bias_scale', C.c_float),
+        ('bias', C.c_void_p), ('sigma', C.c_void_p), ('noise_sigma', C.c_void_p),
+        ('act', C.c_int32), ('sample', C.c_int32),
+        ('seed', C.c_uint64),
+        ('site', C.c_uint32), ('t', C.c_uint32), ('tick', C.c_uint32), ('row0', C.c_uint32), ('tick_off', C.c_uint32),
+        ('ais_kind', C.c_int32),
+        ('ais_a', C.c_float), ('ais_b', C.c_float), ('ais_next', C.c_float), ('ais_lin', C.c_float),
+        ('logw', C.c_void_p), ('logw_len', C.c_int32),
+        ('mean_bf', C.c_void_p), ('mean_rows', C.c_int32), ('mean_ld', C.c_int32),
+        ('state_bf', C.c_void_p), ('state_rows', C.c_int32), ('state_ld', C.c_int32),
+        ('f32', C.c_void_p), ('f32_rows', C.c_int32), ('f32_ld', C.c_int32),
+        ('mode', C.c_int32), ('bn', C.c_int32), ('cluster', C.c_int32), ('units', C.c_int32), ('ctas', C.c_int32),
     ]
 
 
@@ -106,6 +127,7 @@ def load_library(path=None):
         'bm_rbm_metrics': [vp, vp, i32, i32, u64, u32, u32, C.POINTER(dbl)],
         'bm_rbm_get_activation': [vp, C.c_char_p, vp, sz],
         'bm_debug_tc_gemm': [vp, i32, i32, i32, vp, i32, vp, i32, i32, vp, vp, i32, i32, i32, i32, vp],
+        'bm_debug_tc_op': [vp, C.POINTER(TcOpArgs)],
         'bm_dbm_create': [vp, C.POINTER(DbmCfg), C.POINTER(vp)],
         'bm_dbm_set_param': [vp, C.c_char_p, vp, sz], 'bm_dbm_get_param': [vp, C.c_char_p, vp, sz],
         'bm_dbm_init_particles': [vp, u64],
@@ -304,6 +326,89 @@ def debug_tc_gemm(A, B, a_t=False, b_t=False, A2=None, B2=None, neg2=False, spli
                                           K2, p2a, p2b, int(neg2), int(splits), int(force_bn), int(force_cluster),
                                           Cout.ctypes.data))
     return Cout
+
+
+# epilogue modes of the tensor-core kernel (csrc/bm_tc.cu), as debug_tc_op reports them
+TC_MODES = ('GENERIC', 'SIG_BERN_MEAN_STATE', 'SIG_BERN_STATE', 'SIG_MEAN', 'RAW_F32', 'AIS_UNITS', 'AIS_STATE', 'AIS_UNITS_S',
+            'AIS_UNITS_G')
+TC_ACTS = {'linear': 0, 'sigmoid': 1, 'softplus': 2}
+TC_SAMPLES = {None: 0, 'bernoulli': 1, 'gaussian': 2}
+# what debug_tc_op fills its output buffers with before the launch: NaN bit patterns no epilogue produces
+BF16_SENTINEL = 0xFFA5
+F32_SENTINEL = 0xFFC0DEAD
+LOGW_SENTINEL = -1234.5
+
+
+def _round8(n):
+    return (n + 7) // 8 * 8
+
+
+def debug_tc_op(pairs, outputs=('f32',), splits=1, force_bn=0, force_cluster=0, acc_scale=1.0, bias_scale=1.0, bias=None,
+                sigma=None, noise_sigma=None, act='linear', sample=None, seed=0, site=0, t=0, tick=0, row0=0, tick_off=0,
+                ais_kind=0, ais_a=0.0, ais_b=0.0, ais_next=0.0, ais_lin=0.0, logw=None, mean_ld=None, state_ld=None,
+                f32_ld=None, guard_rows=2, ctx=None):
+    """One fused tensor-core op (test hook, bm_debug_tc_op): C = sum over `pairs` of (+/-) A B^T, then the epilogue.
+
+    pairs: 1 or 2 tuples (A, B, a_t, b_t, neg); A is [M,K] (a_t: [K,M]), B is [N,K] (b_t: [K,N]), rounded to bf16 here.
+    outputs: any of 'mean', 'state' (bf16) and 'f32'.  Every output buffer has `guard_rows` rows past M and columns past
+    round_up(N, 8), is filled with the sentinel bit pattern before the launch and is returned whole: 'mean' / 'state' as
+    uint16 bf16 bit patterns [M + guard_rows, ld], 'f32' as float32 [splits, M + guard_rows, ld].  logw (float64 [M]) is
+    added to by the AIS epilogues and returned with one guard entry (LOGW_SENTINEL) past M.  'plan' describes the launch."""
+    ctx = ctx or Context.default()
+    if not 1 <= len(pairs) <= 2:
+        raise ValueError('one or two operand pairs')
+    a = TcOpArgs()
+    keep = []
+    for p, (A, B, a_t, b_t, neg) in enumerate(pairs):
+        A, B = np.asarray(A, dtype=np.float32), np.asarray(B, dtype=np.float32)
+        M, K = (A.shape[1], A.shape[0]) if a_t else A.shape
+        N = B.shape[1] if b_t else B.shape[0]
+        if p == 0:
+            a.M, a.N = M, N
+        elif (M, N) != (a.M, a.N):
+            raise ValueError('the pairs disagree about the output shape')
+        if (B.shape[0] if b_t else B.shape[1]) != K:
+            raise ValueError('A and B of pair {0} disagree about K'.format(p))
+        Ab, Bb = as_bf16(A), as_bf16(B)
+        keep += [Ab, Bb]
+        a.K[p], a.a_t[p], a.b_t[p], a.neg[p] = K, int(bool(a_t)), int(bool(b_t)), int(bool(neg))
+        a.A[p], a.B[p] = Ab.ctypes.data, Bb.ctypes.data
+    a.n_pairs = len(pairs)
+    M, N = a.M, a.N
+    a.splits, a.force_bn, a.force_cluster = int(splits), int(force_bn), int(force_cluster)
+    a.acc_scale, a.bias_scale = float(acc_scale), float(bias_scale)
+    for name, v in (('bias', bias), ('sigma', sigma), ('noise_sigma', noise_sigma)):
+        if v is not None:
+            v = np.ascontiguousarray(v, dtype=np.float32).reshape(N)
+            keep.append(v)
+            setattr(a, name, v.ctypes.data)
+    a.act, a.sample = TC_ACTS[act], TC_SAMPLES[sample]
+    a.seed, a.site, a.t, a.tick, a.row0, a.tick_off = int(seed) & (2 ** 64 - 1), int(site), int(t), int(tick), int(row0), int(tick_off)
+    a.ais_kind, a.ais_a, a.ais_b, a.ais_next, a.ais_lin = int(ais_kind), float(ais_a), float(ais_b), float(ais_next), float(ais_lin)
+    out = {}
+    rows = M + int(guard_rows)
+    if logw is not None:
+        lw = np.empty(M + 1, dtype=np.float64)
+        lw[:M], lw[M] = logw, LOGW_SENTINEL
+        out['logw'] = lw
+        a.logw, a.logw_len = lw.ctypes.data, M + 1
+    for name in outputs:
+        if name in ('mean', 'state'):
+            ld = int((mean_ld if name == 'mean' else state_ld) or _round8(N) + 8)
+            buf = np.full((rows, ld), BF16_SENTINEL, dtype=np.uint16)
+            setattr(a, name + '_bf', buf.ctypes.data)
+            setattr(a, name + '_rows', rows)
+            setattr(a, name + '_ld', ld)
+        elif name == 'f32':
+            ld = int(f32_ld or _round8(N) + 2)
+            buf = np.full((max(1, int(splits)), rows, ld), F32_SENTINEL, dtype=np.uint32).view(np.float32)
+            a.f32, a.f32_rows, a.f32_ld = buf.ctypes.data, rows, ld
+        else:
+            raise ValueError('unknown output ' + repr(name))
+        out[name] = buf
+    check(load_library().bm_debug_tc_op(ctx.handle, C.byref(a)))
+    out['plan'] = dict(mode=TC_MODES[a.mode], bn=a.bn, cluster=a.cluster, units=a.units, ctas=a.ctas)
+    return out
 
 
 def _mask(names):

@@ -9,6 +9,7 @@
 #include "bm_rbm.h"
 #include "bm_peer.h"
 #include <stdlib.h>
+#include <string.h>
 #include <map>
 #include <memory>
 #include <tuple>
@@ -614,5 +615,90 @@ extern "C" int bm_debug_tc_gemm(bm_ctx* hctx, int32_t M, int32_t N, int32_t K, c
         for (int i = 0; i < 24 && h[32 + i]; ++i) fprintf(stderr, " %llu", h[32 + i] - h[0]);
         fprintf(stderr, "\n");
     }
+    BM_API_END
+}
+
+extern "C" int bm_debug_tc_op(bm_ctx* hctx, bm_tc_op_args* a) {
+    BM_API_BEGIN
+    Ctx* ctx = reinterpret_cast<Ctx*>(hctx);
+    BM_REQUIRE(ctx && a && a->M > 0 && a->N > 0 && (a->n_pairs == 1 || a->n_pairs == 2), "bad argument");
+    BM_CUDA(cudaSetDevice(ctx->device));
+    const int M = a->M, N = a->N, n8 = round_up(N, 8);
+    TcGemm g;
+    g.M = M; g.N = N; g.n_pairs = a->n_pairs;
+    // operands: bf16 bit patterns, copied into buffers whose leading dimension is a multiple of 8 (TMA)
+    DevBuf<__nv_bfloat16> ops[4];
+    std::vector<uint16_t> staged;
+    for (int i = 0; i < 2 * g.n_pairs; ++i) {
+        const int pr = i / 2; const bool isA = (i % 2) == 0;
+        const uint16_t* src = isA ? a->A[pr] : a->B[pr];
+        const bool t = (isA ? a->a_t[pr] : a->b_t[pr]) != 0;
+        const int Kp = a->K[pr];
+        BM_REQUIRE(src && Kp > 0, "bad operand");
+        const int mn = isA ? M : N;
+        const int rows = t ? Kp : mn, cols = t ? mn : Kp, ld = round_up(cols, 8);
+        staged.assign((size_t)rows * ld, 0);
+        for (int r = 0; r < rows; ++r) memcpy(&staged[(size_t)r * ld], src + (size_t)r * cols, (size_t)cols * 2);
+        ops[i].ensure(staged.size());
+        BM_CUDA(cudaMemcpyAsync(ops[i].p, staged.data(), staged.size() * 2, cudaMemcpyHostToDevice, ctx->stream));
+        TcMat m; m.ptr = ops[i].p; m.rows = rows; m.cols = cols; m.ld = ld;
+        if (isA) { g.A[pr] = m; g.a_t[pr] = t; g.neg[pr] = a->neg[pr] != 0; } else { g.B[pr] = m; g.b_t[pr] = t; }
+        g.K[pr] = Kp;
+    }
+    g.splits = a->splits > 0 ? a->splits : 1;
+    g.force_bn = a->force_bn; g.force_cluster = a->force_cluster;
+    // epilogue vectors
+    DevBuf<float> vec[3];
+    const float* vsrc[3] = {a->bias, a->sigma, a->noise_sigma};
+    for (int i = 0; i < 3; ++i) {
+        if (!vsrc[i]) continue;
+        vec[i].ensure((size_t)N);
+        BM_CUDA(cudaMemcpyAsync(vec[i].p, vsrc[i], (size_t)N * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    }
+    g.bias = vec[0].p; g.sigma = vec[1].p; g.noise_sigma = vec[2].p;
+    g.acc_scale = a->acc_scale; g.bias_scale = a->bias_scale;
+    g.act = a->act; g.sample = a->sample;
+    g.rng = make_rng(a->seed, a->site, a->t, a->tick, a->row0);
+    g.tick_off = a->tick_off;
+    g.ais_kind = a->ais_kind; g.ais_a = a->ais_a; g.ais_b = a->ais_b; g.ais_next = a->ais_next; g.ais_lin = a->ais_lin;
+    // outputs and log-weights: whole buffers in, whole buffers out
+    DevBuf<double> logw;
+    if (a->logw) {
+        BM_REQUIRE(a->logw_len > M, "log-weights need a guard entry past M");
+        logw.ensure((size_t)a->logw_len);
+        BM_CUDA(cudaMemcpyAsync(logw.p, a->logw, (size_t)a->logw_len * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+        g.ais_logw = logw.p;
+    }
+    DevBuf<__nv_bfloat16> mean, state;
+    DevBuf<float> f32;
+    const size_t mean_n = (size_t)a->mean_rows * a->mean_ld, state_n = (size_t)a->state_rows * a->state_ld;
+    const size_t f32_n = (size_t)g.splits * a->f32_rows * a->f32_ld;
+    if (a->mean_bf) {
+        BM_REQUIRE(a->mean_rows > M && a->mean_ld > n8 && a->mean_ld % 8 == 0, "bf16 means need guard rows and columns");
+        mean.ensure(mean_n);
+        BM_CUDA(cudaMemcpyAsync(mean.p, a->mean_bf, mean_n * 2, cudaMemcpyHostToDevice, ctx->stream));
+        g.out_mean_bf = mean.p; g.ld_mean_bf = a->mean_ld;
+    }
+    if (a->state_bf) {
+        BM_REQUIRE(a->state_rows > M && a->state_ld > n8 && a->state_ld % 8 == 0, "bf16 states need guard rows and columns");
+        state.ensure(state_n);
+        BM_CUDA(cudaMemcpyAsync(state.p, a->state_bf, state_n * 2, cudaMemcpyHostToDevice, ctx->stream));
+        g.out_state_bf = state.p; g.ld_state_bf = a->state_ld;
+    }
+    if (a->f32) {
+        BM_REQUIRE(a->f32_rows > M && a->f32_ld > n8, "fp32 outputs need guard rows and columns");
+        f32.ensure(f32_n);
+        BM_CUDA(cudaMemcpyAsync(f32.p, a->f32, f32_n * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+        g.out_f32 = f32.p; g.ld_f32 = a->f32_ld;
+        g.split_stride = (size_t)a->f32_rows * a->f32_ld;
+    }
+    TcPlan plan;
+    launch_tc_gemm(ctx, g, &plan);          // refuses an op it does not run before launching anything
+    a->mode = plan.mode; a->bn = plan.bn; a->cluster = plan.cluster; a->units = plan.units; a->ctas = plan.ctas;
+    if (a->mean_bf) BM_CUDA(cudaMemcpyAsync(a->mean_bf, mean.p, mean_n * 2, cudaMemcpyDeviceToHost, ctx->stream));
+    if (a->state_bf) BM_CUDA(cudaMemcpyAsync(a->state_bf, state.p, state_n * 2, cudaMemcpyDeviceToHost, ctx->stream));
+    if (a->f32) BM_CUDA(cudaMemcpyAsync(a->f32, f32.p, f32_n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    if (a->logw) BM_CUDA(cudaMemcpyAsync(a->logw, logw.p, (size_t)a->logw_len * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    BM_CUDA(cudaStreamSynchronize(ctx->stream));
     BM_API_END
 }

@@ -333,7 +333,9 @@ __device__ __forceinline__ void mma_chunk_any(int cfg, int bn16, float (&acc)[NB
     }
 }
 
-__device__ __forceinline__ float fast_softplus(float x) { return fmaxf(x, 0.f) + __logf(1.0f + __expf(-fabsf(x))); }
+// log1pf, not __logf(1 + e): 1 + e rounds away the relative precision of e, so softplus(x) for x below about -10 (the
+// result is then e itself) was off by several bf16 ulps
+__device__ __forceinline__ float fast_softplus(float x) { return fmaxf(x, 0.f) + log1pf(__expf(-fabsf(x))); }
 // sigmoid(x) = 1 / (1 + 2^(-x log2 e)): ex2.approx + rcp.approx keep the *relative* error of small
 // probabilities at ~1e-7 (tanh.approx would not)
 __device__ __forceinline__ float sigmoid_from_neg_log2(float t) {   // t = -x * log2(e)
@@ -1098,6 +1100,16 @@ static void fill_phase(Ctx* ctx, const TcGemm& g, int cluster, TcPhase& ph) {
     BM_REQUIRE(!g.out_state_bf || (g.ld_state_bf % 8 == 0), "bf16 output leading dimension must be a multiple of 8");
 }
 
+// what a single-op launch of the filled descriptor `ph` runs: one unit per (row group, column block, split), and as many
+// CTA pairs (CTAs) as there are units, at most one per SM (do_launch sizes the grid the same way)
+static TcPlan tc_describe(const TcPhase& ph, int cluster, int sm_count) {
+    TcPlan p;
+    p.mode = ph.l.mode; p.bn = ph.l.BN; p.cluster = cluster;
+    p.units = ph.l.m_groups * ph.l.n_tiles * ph.l.splits;
+    p.ctas = std::min(p.units, sm_count / cluster) * cluster;
+    return p;
+}
+
 // The ops' descriptors (minus tensor maps) go to constant memory, stream-ordered before the launch;
 // skipped when the bank already holds exactly this image (the common case: the same program every step).
 static void upload_ops(Ctx* ctx, const TcPhase* ph, int n) {
@@ -1180,7 +1192,7 @@ static double gemm_flops(const TcGemm& g) {
     return 2.0 * g.M * g.N * k_total;
 }
 
-void launch_tc_gemm(Ctx* ctx, const TcGemm& g) {
+void launch_tc_gemm(Ctx* ctx, const TcGemm& g, TcPlan* plan) {
     const int m_tiles = (g.M + BM - 1) / BM;
     int cluster = g.force_cluster > 0 ? g.force_cluster : (m_tiles >= 2 ? 2 : 1);
     BM_REQUIRE(cluster == 1 || cluster == 2, "cluster must be 1 or 2");
@@ -1198,6 +1210,7 @@ void launch_tc_gemm(Ctx* ctx, const TcGemm& g) {
     L.dbg = g.dbg;
     L.mant_mask = 0x007FFFFFu; L.one_bits = 0x3F800000u;
     L.epoch = 1; L.poll_ns = 64; L.epi_ns = 128;
+    if (plan) *plan = tc_describe(L.inl, cluster, ctx->sm_count);
     upload_ops(ctx, &L.inl, 1);
     do_launch(ctx, L, cluster, gemm_flops(g), L.inl.l.BN);
 }

@@ -65,7 +65,11 @@ struct TcGemm {
 };
 enum : int { LANE_CHAIN = 0, LANE_SPARE = 1, LANE_ALL = 2 };
 
-void launch_tc_gemm(Ctx* ctx, const TcGemm& g);
+// what a single-op launch runs (tc_describe in bm_tc.cu): the epilogue mode, the tile width, the row grouping (1 or 2), the
+// number of units and the CTAs of the grid
+struct TcPlan { int mode, bn, cluster, units, ctas; };
+// `plan` (nullable) receives the description of the launch before it is issued
+void launch_tc_gemm(Ctx* ctx, const TcGemm& g, TcPlan* plan = nullptr);
 // number of (row-block pair, column block, split) units the tile heuristic cuts `g` into inside a program
 int tc_plan_units(Ctx* ctx, const TcGemm& g);
 

@@ -208,6 +208,42 @@ int  bm_debug_tc_gemm(bm_ctx* ctx, int32_t M, int32_t N, int32_t K, const float*
                       const float* B, int32_t b_t, int32_t K2, const float* A2, const float* B2,
                       int32_t neg2, int32_t splits, int32_t force_bn, int32_t force_cluster, float* C);
 
+/* ---- test hook: ONE fused tensor-core op, every output returned whole --------------------
+ * C[M,N] = sum_p (+/-) A_p * B_p^T over n_pairs (1 or 2) operand pairs given as bf16 bit patterns:
+ * A_p is [M,K_p] row-major (a_t[p]: [K_p,M]), B_p is [N,K_p] (b_t[p]: [K_p,N]); then the op's epilogue
+ *   pre = acc_scale * C * sigma[n] + bias_scale * bias[n],  mean = act(pre),  state = sample(mean)
+ * with the draws of element (r, c) taken from Philox (seed, site | t << 8, tick + tick_off, row0 + r) as in the engine.
+ * ais_kind 1 / 2 select the AIS epilogues (see csrc/bm_tc_desc.h); logw [logw_len] is added to and returned.
+ * Outputs are optional (NULL: not written) and given WHOLE, as the caller filled them: each buffer is copied to the device,
+ * the op writes its [M, N] window (split s of a split-K op: f32 + s * f32_rows * f32_ld), and the whole buffer comes back,
+ * so that a test sees anything written outside the window.  Each needs a guard row (rows > M) and guard columns
+ * (ld > round_up(N, 8)); bf16 leading dimensions are multiples of 8, the fp32 one may be odd.
+ * On return mode, bn, cluster, units and ctas describe the launch: the epilogue mode the op ran with, the tile width, the
+ * row grouping (1: a CTA per 128-row block, 2: CTA pairs per 256-row group), the number of units and the CTAs of the grid.
+ * An op the engine does not run is refused with BM_EINVAL before anything is launched. */
+typedef struct bm_tc_op_args {
+    int32_t M, N, n_pairs;
+    int32_t K[2], a_t[2], b_t[2], neg[2];
+    const uint16_t* A[2];
+    const uint16_t* B[2];
+    int32_t splits, force_bn, force_cluster;
+    float acc_scale, bias_scale;
+    const float* bias;                     /* [N] or NULL (host) */
+    const float* sigma;                    /* [N] or NULL */
+    const float* noise_sigma;              /* [N] or NULL */
+    int32_t act, sample;                   /* 0 linear, 1 sigmoid, 2 softplus;  0 none, 1 Bernoulli, 2 Gaussian */
+    uint64_t seed;
+    uint32_t site, t, tick, row0, tick_off;
+    int32_t ais_kind;
+    float ais_a, ais_b, ais_next, ais_lin;
+    double* logw;          int32_t logw_len;
+    uint16_t* mean_bf;     int32_t mean_rows, mean_ld;
+    uint16_t* state_bf;    int32_t state_rows, state_ld;
+    float* f32;            int32_t f32_rows, f32_ld;
+    int32_t mode, bn, cluster, units, ctas;          /* out: what was launched */
+} bm_tc_op_args;
+int  bm_debug_tc_op(bm_ctx* ctx, bm_tc_op_args* args);
+
 #ifdef __cplusplus
 }
 #endif
