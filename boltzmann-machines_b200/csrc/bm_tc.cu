@@ -995,19 +995,22 @@ static CUtensorMap make_map(const TcMat& m, int box0, int box1) {
 
 struct TilePick { int bn, cluster; };
 
-static TilePick pick_tile(int N, int m_tiles, int splits, int chunks, int sms, int force_cluster) {
-    // Tile width BN (64 or 128: whole 64-column wgmma blocks and TMA-store granules) and row grouping (CTAs
+static TilePick pick_tile(int N, int m_tiles, int splits, int chunks, int sms, int force_cluster, int max_bn) {
+    // Tile width BN (64, 128 or 256: whole 64-column wgmma blocks and TMA-store granules) and row grouping (CTAs
     // taking one 128-row block each, or pairs taking a 256-row group).  Cycle model per CTA:
     // waves * chunks * max(mma, ingest) + epilogue of the last tile, with the tensor cores at ~2048 bf16
-    // MACs/clk per SM (989 TFLOP/s dense over 132 SMs) and L2 ingest assumed at ~32 B/clk per SM (not measured).
+    // MACs/clk per SM (989 TFLOP/s dense over 132 SMs) and operand ingest at ~32 B/clk per SM (measured on an H100 at
+    // 64, 128 and 256 columns alike, DESIGN 5.1): every width is ingest-bound, and a wider tile reads the A tile once
+    // for more columns -- 48 KiB per 1024 MMA cycles at BN = 256 against 32 KiB per 512 at BN = 128.
     TilePick best{64, 1};
     double best_cost = 1e30;
     for (int c = 1; c <= 2; ++c) {
         if (force_cluster && c != force_cluster) continue;
         if (!force_cluster && c == 2 && m_tiles < 2) break;
         const int slots = sms / c * c;                 // CTAs of the grid
-        // (192 / 256 and widths of 16-column steps are reachable through force_bn only: a 256-wide tile leaves 3 ring stages)
-        for (int bn = 64; bn <= 128; bn += 64) {
+        // (192 and widths of 16-column steps are reachable through force_bn only; a 256-wide tile leaves 3 ring stages,
+        // which keep up with the ingest rate)
+        for (int bn = 64; bn <= max_bn; bn *= 2) {
             const int nt = (N + bn - 1) / bn;
             const int m_groups = (m_tiles + c - 1) / c;
             const long units = (long)m_groups * c * nt * splits;
@@ -1050,7 +1053,10 @@ static void fill_phase(Ctx* ctx, const TcGemm& g, int cluster, TcPhase& ph) {
     int chunks_total = 0;
     for (int i = 0; i < g.n_pairs; ++i) chunks_total += (g.K[i] + BK - 1) / BK;
     const int nsplit = g.splits > 0 ? g.splits : 1;
-    TilePick tp = pick_tile(g.N, m_tiles, nsplit, (chunks_total + nsplit - 1) / nsplit, ctx->sm_count, cluster);
+    // AIS ops stay at 128 columns or less: their epilogues (a softplus difference or a series per element, an fp64 atomic per
+    // row and tile) cost more than the model's per-column term, and an AIS ladder of the cfg4 DBM measured 7% slower at 256
+    const int max_bn = g.ais_kind ? 128 : MAX_BN;
+    TilePick tp = pick_tile(g.N, m_tiles, nsplit, (chunks_total + nsplit - 1) / nsplit, ctx->sm_count, cluster, max_bn);
     if (g.force_bn > 0) tp.bn = g.force_bn;
     BM_REQUIRE(tp.cluster == cluster, "tile picker returned another row grouping");
     bool b_mn = false;
@@ -1298,7 +1304,11 @@ void launch_tc_program(Ctx* ctx, TcProgram& prog, RngKey rng, int batch_row) {
                     ph[i].l.dep_gran_row = pj.n_tiles * pj.gran_per_tile;
                     ph[i].l.dep_chunk_need = cluster;              // the publisher of each CTA of the producing pair
                     // K chunk c = columns [64c, 64c+64) of the producer's output: the granule(s) holding its
-                    // first and last column; consumed in the order the producer's epilogues finish them
+                    // first and last column; consumed in the order the producer's epilogues finish them.  A 256-wide
+                    // producer is consumed in the order of a 128-wide one (granules 0 and 2 of a tile before 1 and 3):
+                    // the K order is the summation order of the consumer's accumulators, and keeping it lets the tile
+                    // picker choose between 128 and 256 columns without changing a single result bit.
+                    const int order_cols = pj.BN == 256 ? 128 : pj.BN;
                     std::vector<std::pair<int, int>> order;
                     for (int c = 0; c < kchunks; ++c) {
                         const int col_a = 64 * c, col_b = std::min(64 * c + 63, pj.N - 1);
@@ -1306,7 +1316,7 @@ void launch_tc_program(Ctx* ctx, TcProgram& prog, RngKey rng, int batch_row) {
                         const int ga = (col_a - ta * pj.BN) / GRAN_COLS, gb = (col_b - tb * pj.BN) / GRAN_COLS;
                         ph[i].l.k_dep_a[c] = (unsigned char)(ta * pj.gran_per_tile + ga);
                         ph[i].l.k_dep_b[c] = (unsigned char)(tb * pj.gran_per_tile + gb);
-                        order.push_back(std::make_pair(std::max(ga, gb), c));
+                        order.push_back(std::make_pair(std::max(col_a % order_cols, col_b % order_cols) / GRAN_COLS, c));
                     }
                     std::stable_sort(order.begin(), order.end());
                     for (int c = 0; c < kchunks; ++c) ph[i].l.k_order[c] = (unsigned char)order[c].second;
