@@ -527,9 +527,18 @@ __device__ __forceinline__ float pair_body(const EpiCtx& c, float v0, float v1, 
     return ais_part;
 }
 
+// Register k of accumulator block j, j known only at run time: a select chain, so the granule loop below can stay rolled
+// without moving the accumulators out of registers.
+__device__ __forceinline__ float acc_at(const float (&acc)[NB_MAX][32], int j, int k) {
+    static_assert(NB_MAX == 4, "one select per accumulator block");
+    return j == 0 ? acc[0][k] : (j == 1 ? acc[1][k] : (j == 2 ? acc[2][k] : acc[3][k]));
+}
+
 // The warpgroup's share of a tile, granule (64 columns = one accumulator block) by granule: each granule of each bf16
 // output takes the next buffer of the staging FIFO, is written by the 8 consumer warps and announced on the buffer's
 // `full` barrier; the publisher warps store it with TMA and publish it to the other SMs.
+// The granule loop is rolled: unrolled, every mode's epilogue held four copies of its 8-block body (32 inlined Philox blocks
+// for a sampling mode), and the first unit of each mode in a launch spent most of its epilogue fetching that code.
 template <int MODE>
 __device__ __forceinline__ void epilogue_tile(const EpiCtx& c, const float (&acc)[NB_MAX][32]) {
     typedef EpiCfg<MODE> E;
@@ -552,9 +561,8 @@ __device__ __forceinline__ void epilogue_tile(const EpiCtx& c, const float (&acc
     const uint32_t off0 = (uint32_t)c.r0 * 128u + (uint32_t)q * 4u, off1 = off0 + 8u * 128u;
     float ais0 = 0.f, ais1 = 0.f;
     uint32_t seq = *c.seq;
-#pragma unroll
-    for (int j = 0; j < NB_MAX; ++j) {
-        if (j >= nb) break;
+#pragma unroll 1
+    for (int j = 0; j < nb; ++j) {
         uint32_t smem_mean = 0, smem_state = 0;
         int b_mean = 0, b_state = 0;
         if (do_mean) {
@@ -588,8 +596,8 @@ __device__ __forceinline__ void epilogue_tile(const EpiCtx& c, const float (&acc
                 }
                 const float2 b2 = *reinterpret_cast<const float2*>(c.sbias + j * GRAN_COLS + cl);
                 uint32_t mp0, sp0, mp1, sp1;
-                ais0 += pair_body<MODE>(c, acc[j][4 * i], acc[j][4 * i + 1], w0f, w0s, b2.x, b2.y, n, c.m0, ok0, out_f32, f32_vec, mp0, sp0);
-                ais1 += pair_body<MODE>(c, acc[j][4 * i + 2], acc[j][4 * i + 3], w1f, w1s, b2.x, b2.y, n, m1, ok1, out_f32, f32_vec, mp1, sp1);
+                ais0 += pair_body<MODE>(c, acc_at(acc, j, 4 * i), acc_at(acc, j, 4 * i + 1), w0f, w0s, b2.x, b2.y, n, c.m0, ok0, out_f32, f32_vec, mp0, sp0);
+                ais1 += pair_body<MODE>(c, acc_at(acc, j, 4 * i + 2), acc_at(acc, j, 4 * i + 3), w1f, w1s, b2.x, b2.y, n, m1, ok1, out_f32, f32_vec, mp1, sp1);
                 // columns past N and rows past M are written to the staging buffer too: the TMA store clips them
                 const uint32_t u = (((uint32_t)i ^ swz) << 4);
                 if (do_mean) { sts32(smem_mean + off0 + u, mp0); sts32(smem_mean + off1 + u, mp1); }
