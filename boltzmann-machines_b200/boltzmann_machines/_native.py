@@ -27,7 +27,7 @@ EXPORTS = (
     'bm_ctx_launch_count', 'bm_ctx_profile_tc', 'bm_ctx_profile_read', 'bm_comm_unique_id', 'bm_ctx_comm_init',
     'bm_rbm_create', 'bm_rbm_destroy', 'bm_rbm_set_param', 'bm_rbm_get_param', 'bm_rbm_init_weights',
     'bm_rbm_train_step', 'bm_rbm_set_data', 'bm_rbm_train_step_at', 'bm_rbm_train_epoch', 'bm_rbm_train_epoch_u8', 'bm_rbm_train_epoch_bf16', 'bm_rbm_transform', 'bm_rbm_metrics',
-    'bm_rbm_get_activation', 'bm_debug_tc_gemm', 'bm_debug_tc_op',
+    'bm_rbm_get_activation', 'bm_debug_tc_gemm', 'bm_debug_tc_op', 'bm_rbm_debug_tc_plan',
     'bm_dbm_create', 'bm_dbm_destroy', 'bm_dbm_set_param', 'bm_dbm_get_param', 'bm_dbm_init_particles',
     'bm_dbm_train_step', 'bm_dbm_val_metrics', 'bm_dbm_transform', 'bm_dbm_reconstruct', 'bm_dbm_log_proba',
     'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows',
@@ -88,6 +88,11 @@ class TcOpArgs(C.Structure):
     ]
 
 
+class TcOpPlan(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ('launch', 'mode', 'bn', 'm_groups', 'n_tiles', 'splits', 'pair_begin', 'pair_count',
+                                         'follows_granules')]
+
+
 _lib = None
 
 
@@ -128,6 +133,7 @@ def load_library(path=None):
         'bm_rbm_get_activation': [vp, C.c_char_p, vp, sz],
         'bm_debug_tc_gemm': [vp, i32, i32, i32, vp, i32, vp, i32, i32, vp, vp, i32, i32, i32, i32, vp],
         'bm_debug_tc_op': [vp, C.POINTER(TcOpArgs)],
+        'bm_rbm_debug_tc_plan': [vp, C.POINTER(TcOpPlan), i32, C.POINTER(i32)],
         'bm_dbm_create': [vp, C.POINTER(DbmCfg), C.POINTER(vp)],
         'bm_dbm_set_param': [vp, C.c_char_p, vp, sz], 'bm_dbm_get_param': [vp, C.c_char_p, vp, sz],
         'bm_dbm_init_particles': [vp, u64],
@@ -571,6 +577,23 @@ class CudaRBM(object):
         a = np.empty((rows, n), dtype=dt)
         check(self._lib.bm_rbm_get_activation(self.handle, name.encode(), a.ctypes.data, a.nbytes))
         return a
+
+    def debug_tc_plan(self):
+        """(test hook, bm_rbm_debug_tc_plan) the ops of the last tensor-core program, in program order across its launches:
+        one dict per op with launch, mode (a TC_MODES name), bn, m_groups, n_tiles, splits, units, pair_begin, pair_count and
+        follows_granules (the op waits for its producer's 64-column granules one by one)."""
+        n = C.c_int32(0)
+        check(self._lib.bm_rbm_debug_tc_plan(self.handle, None, 0, C.byref(n)))
+        recs = (TcOpPlan * max(1, n.value))()
+        check(self._lib.bm_rbm_debug_tc_plan(self.handle, recs, n.value, C.byref(n)))
+        out = []
+        for r in recs[:n.value]:
+            d = {f: int(getattr(r, f)) for f, _ in TcOpPlan._fields_}
+            d['mode'] = TC_MODES[d['mode']]
+            d['follows_granules'] = bool(d['follows_granules'])
+            d['units'] = d['m_groups'] * d['n_tiles'] * d['splits']
+            out.append(d)
+        return out
 
     def close(self):
         if getattr(self, 'handle', None):

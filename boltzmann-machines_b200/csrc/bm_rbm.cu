@@ -109,5 +109,12 @@ int bm_rbm_get_activation(bm_rbm* h, const char* name, void* host, size_t bytes)
     RBM(h)->get_activation(name, host, bytes);
     BM_API_END
 }
+int bm_rbm_debug_tc_plan(bm_rbm* h, bm_tc_op_plan* out, int32_t cap, int32_t* n_ops) {
+    BM_API_BEGIN RBM_ENTER(h) BM_REQUIRE(n_ops && (out || cap == 0) && cap >= 0, "bad argument");
+    const std::vector<bm_tc_op_plan>& plan = RBM(h)->tc_plan();
+    *n_ops = (int32_t)plan.size();
+    for (size_t i = 0; i < plan.size() && (int32_t)i < cap; ++i) out[i] = plan[i];
+    BM_API_END
+}
 
 }  // extern "C"

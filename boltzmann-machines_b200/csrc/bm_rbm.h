@@ -43,6 +43,8 @@ struct RbmBase {
     virtual void transform(const void* X, int rows, int k, uint64_t seed, uint32_t tick, void* H_out) = 0;
     virtual void metrics(const void* X, int rows, int k, uint64_t seed, uint32_t tick, uint32_t mask, double* out) = 0;
     virtual void get_activation(const char* name, void* host, size_t bytes) = 0;
+    // test hook (bm_rbm_debug_tc_plan): the ops of the last tensor-core program
+    virtual const std::vector<bm_tc_op_plan>& tc_plan() const { throw Error(BM_EINVAL, "this engine runs no tensor-core program"); }
 };
 
 // ------------------------------------------------------------------------------------------

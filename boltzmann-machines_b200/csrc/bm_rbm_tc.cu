@@ -35,6 +35,7 @@ struct RbmTC : RbmSimt<float> {
     // cached programs, keyed by (rows, k, with_dw, input buffer is the resident dataset)
     std::map<std::tuple<int, int, int, int>, std::unique_ptr<TcProgram>> progs;
     int dw_splits = 1, v_splits = 1;
+    std::vector<bm_tc_op_plan> last_plan;          // the ops of the last run_program, all its launches (bm_rbm_debug_tc_plan)
     static constexpr int PROGRAM_OPS = 90;      // ops per launch (the kernel's descriptor table holds 96)
     PeerExchange peer;             // data parallelism over NVLink peer memory (inactive on one rank / without peer access)
     // The batch buffers (X, v_k) carry two constant columns behind their V data columns -- (1, 0) for X, (1, 1) for v_k --
@@ -218,6 +219,7 @@ struct RbmTC : RbmSimt<float> {
     // (base_rbm.py:447-448) -- as ONE persistent launch.
     void run_program(int rows, int k, bool with_dw, uint64_t seed, uint32_t tick, uint32_t row0) {
         BM_REQUIRE(k >= 1, "n_gibbs_steps must be >= 1");
+        last_plan.clear();
         const bool resident = X_mode != 0;           // the input is addressed through the launch's batch cursor
         auto key = std::make_tuple(rows, k, with_dw ? 1 : 0, X_mode);
         std::unique_ptr<TcProgram>& slot = progs[key];
@@ -360,7 +362,7 @@ struct RbmTC : RbmSimt<float> {
             }
         }
         if ((int)ops.size() <= PROGRAM_OPS) {
-            if (!ops.empty()) launch_tc_program(ctx, prog, make_rng(seed, 0, 0, tick, row0), resident ? X_row0 : 0);
+            if (!ops.empty()) launch_tc_program(ctx, prog, make_rng(seed, 0, 0, tick, row0), resident ? X_row0 : 0, &last_plan);
         } else {
             // a chain longer than one program holds (CD-k with 2k + 3 > 96 ops; the reference has no such limit,
             // base_rbm.py:386-405): consecutive launches of up to PROGRAM_OPS ops -- a dependency on an op of an earlier launch is
@@ -379,7 +381,9 @@ struct RbmTC : RbmSimt<float> {
                     g.n_deps = n;
                     if (g.lane == LANE_SPARE) g.lane = LANE_ALL;
                 }
-                launch_tc_program(ctx, *part, make_rng(seed, 0, 0, tick, row0), resident ? X_row0 : 0);
+                const size_t first = last_plan.size();
+                launch_tc_program(ctx, *part, make_rng(seed, 0, 0, tick, row0), resident ? X_row0 : 0, &last_plan);
+                for (size_t i = first; i < last_plan.size(); ++i) last_plan[i].launch = (int32_t)(c - 1);
             }
         }
         last_was_tc = true;
@@ -511,6 +515,8 @@ struct RbmTC : RbmSimt<float> {
         if (mask & (BM_METRIC_PLL | BM_METRIC_FREE_ENERGY)) ensure_fp32_input(rows);
         run_metrics(mask, rows, seed, tick, 0, out);
     }
+
+    const std::vector<bm_tc_op_plan>& tc_plan() const override { return last_plan; }
 
     void get_activation(const char* name, void* host, size_t bytes) override {
         if (!last_was_tc) { RbmSimt<float>::get_activation(name, host, bytes); return; }

@@ -1240,7 +1240,7 @@ TcProgram::~TcProgram() {
     if (dev_counters) cudaFree(dev_counters);
 }
 
-void launch_tc_program(Ctx* ctx, TcProgram& prog, RngKey rng, int batch_row) {
+void launch_tc_program(Ctx* ctx, TcProgram& prog, RngKey rng, int batch_row, std::vector<bm_tc_op_plan>* plan) {
     const int n = (int)prog.ops.size();
     BM_REQUIRE(n >= 1 && n <= MAX_PHASES, "a program holds 1..96 ops");
     const int cluster = 2;            // programs always run on CTA pairs (all CTAs walk one unit list)
@@ -1386,6 +1386,15 @@ void launch_tc_program(Ctx* ctx, TcProgram& prog, RngKey rng, int batch_row) {
         prog.epoch = 0;
         throw;
     }
+    if (plan)
+        for (int i = 0; i < n; ++i) {
+            const TcPhaseLite& p = ph[i].l;
+            bm_tc_op_plan r{};
+            r.mode = p.mode; r.bn = p.BN; r.m_groups = p.m_groups; r.n_tiles = p.n_tiles; r.splits = p.splits;
+            r.pair_begin = p.pair_begin; r.pair_count = p.pair_count;
+            r.follows_granules = p.dep_chunk_ctr != nullptr;
+            plan->push_back(r);
+        }
     if (dbg) {
         --dbg_left;
         unsigned long long h[1024];

@@ -87,8 +87,9 @@ struct TcProgram {
     int chain_units = -1;                       // largest unit count of the chain ops (planned once by the owner)
     ~TcProgram();
 };
-// seed/tick/row0 of `rng` are shared by all ops; batch_row shifts the ops' a_batch operands
-void launch_tc_program(Ctx* ctx, TcProgram& prog, RngKey rng, int batch_row);
+// seed/tick/row0 of `rng` are shared by all ops; batch_row shifts the ops' a_batch operands.  `plan` (nullable, tests)
+// receives one record per op of the launch, appended once the launch was issued (its `launch` field is left 0).
+void launch_tc_program(Ctx* ctx, TcProgram& prog, RngKey rng, int batch_row, std::vector<bm_tc_op_plan>* plan = nullptr);
 
 // helpers on bf16 activations
 void launch_f32_to_bf16(Ctx* ctx, const float* src, int lds, __nv_bfloat16* dst, int ldd, int rows, int cols);

@@ -244,6 +244,20 @@ typedef struct bm_tc_op_args {
 } bm_tc_op_args;
 int  bm_debug_tc_op(bm_ctx* ctx, bm_tc_op_args* args);
 
+/* ---- test hook: how the last tensor-core program of an RBM was planned -----------------------
+ * One record per op of the last chain the engine ran (train_step, train_step_at, train_epoch's last batch, transform,
+ * metrics), in program order across all the launches a long chain is cut into.  Read-only: decoded from the descriptors
+ * the launch uploaded.  *n_ops receives the number of ops; at most `cap` records are written.  BM_EINVAL for an engine
+ * that runs no tensor-core program. */
+typedef struct bm_tc_op_plan {
+    int32_t launch;                        /* 0, 1, ...: which launch of the chain ran this op */
+    int32_t mode, bn;                      /* epilogue mode (as bm_tc_op_args), tile width */
+    int32_t m_groups, n_tiles, splits;     /* 256-row groups, column tiles, K splits: units = their product */
+    int32_t pair_begin, pair_count;        /* the CTA pairs that run the op's units */
+    int32_t follows_granules;              /* 1: waits for its producer's 64-column granules one by one */
+} bm_tc_op_plan;
+int  bm_rbm_debug_tc_plan(bm_rbm* rbm, bm_tc_op_plan* out, int32_t cap, int32_t* n_ops);
+
 #ifdef __cplusplus
 }
 #endif

@@ -34,3 +34,30 @@ def test_small_op_keeps_narrow_tiles(sim):
     p = plan_of(256, 130, 64, False, False)
     assert p['bn'] == 64, p
     clean(sim)
+
+
+def test_headline_program_plan(sim):
+    """The program of one cfg2 training step, as the engine plans it (launches recorded, not interpreted): h0, five pairs of
+    chain half-steps and the two statistics ops in one launch; every chain op 256 columns wide on the first 64 CTA pairs and
+    following its producer granule by granule; the statistics split over K on all 66 pairs."""
+    from boltzmann_machines import _native
+    V, H, B, k = 784, 1024, 4096, 5
+    sim.fakecuda_reset()
+    sim.fakecuda_set_execute(0)
+    eng = _native.CudaRBM(dict(n_visible=V, n_hidden=H, v_kind='bernoulli', h_kind='bernoulli', dtype='float32', compute='bf16',
+                               l2=1e-5, sample_v=False, sample_h=True, max_batch=B))
+    eng.init_normal_W(0.01, 1337)
+    eng.train_step((np.random.RandomState(3).rand(B, V) < 0.13).astype(np.float32), 0.05, 0.5, k, 7, 0)
+    plan = eng.debug_tc_plan()
+    eng.close()
+    chain = plan[:1 + 2 * k]
+    modes = ['SIG_BERN_MEAN_STATE'] + ['SIG_MEAN', 'SIG_BERN_STATE'] * (k - 1) + ['SIG_MEAN', 'SIG_MEAN']
+    assert [p['mode'] for p in chain] == modes, plan
+    assert len(plan) == len(chain) + 2 and all(p['launch'] == 0 for p in plan), plan
+    for i, p in enumerate(chain):
+        assert (p['bn'], p['m_groups'], p['n_tiles'], p['splits']) == (256, 16, 4, 1), (i, p)
+        assert (p['pair_begin'], p['pair_count'], p['follows_granules']) == (0, 64, i > 0), (i, p)
+    for p in plan[len(chain):]:
+        assert p['mode'] == 'RAW_F32' and p['splits'] > 1 and not p['follows_granules'], p
+        assert (p['pair_begin'], p['pair_count']) == (0, 66), p
+    clean(sim)
