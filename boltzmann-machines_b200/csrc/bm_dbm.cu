@@ -692,8 +692,8 @@ int bm_dbm_create(bm_ctx* hctx, const bm_dbm_cfg* cfg, bm_dbm** out) {
     BM_REQUIRE(cfg->n_particles > 0 && cfg->batch_size > 0, "n_particles and batch_size must be positive");
     BM_REQUIRE(cfg->v_kind != BM_UNIT_GAUSSIAN || cfg->sigma, "gaussian visible layer needs sigma");
     BM_CUDA(cudaSetDevice(ctx->device));
-    // BM_COMPUTE_BF16 (opt-in): float32 models with Bernoulli hidden layers run their GEMMs on the tensor cores; every other
-    // combination keeps the storage-precision CUDA-core engine (as bm_rbm_create does for unit kinds the
+    // BM_COMPUTE_BF16 (the Python mirror's default): float32 models with Bernoulli hidden layers run their GEMMs on the tensor
+    // cores; every other combination keeps the storage-precision CUDA-core engine (as bm_rbm_create does for unit kinds the
     // tensor-core epilogue does not implement)
     DbmBase* d;
     if (cfg->dtype == BM_DTYPE_F64) d = new Dbm<double>(ctx, *cfg);

@@ -12,34 +12,20 @@
 //   softplus(b z) - softplus(a z) = log1p(sigmoid(a z) * expm1((b - a) z)),
 // which is exact to fp32 rounding of a SMALL quantity (no cancellation between two O(1) softplus values).
 //
-// STATUS: opt-in (bm_dbm_cfg.compute = BM_COMPUTE_BF16; the Python mirror passes it only when asked:
-// DBM(..., compute='bf16') or BM_DBM_COMPUTE=bf16).  The default DBM engine is the fp32 CUDA-core one.
+// STATUS: the default engine of float32 DBMs (bm_dbm_cfg.compute = BM_COMPUTE_BF16, which the Python mirror passes unless
+// compute='fp32' or BM_DBM_COMPUTE / BM_COMPUTE = fp32 asks for the storage-precision CUDA-core engine).  Models it does not
+// support (DbmTC::supports) run on that engine.
 #pragma once
 #include <map>
 #include <memory>
 #include <utility>
 #include <tuple>
-#include <stdlib.h>
 
 namespace bm {
 
 typedef __nv_bfloat16 bf16_t;
 
 static inline int dbm_round_up(int x, int m) { return (x + m - 1) / m * m; }
-
-// max |a - b| over a [rows, cols] window of two bf16 matrices (leading dimensions lda / ldb)
-__global__ void max_abs_diff_bf16_kernel(const bf16_t* __restrict__ a, int lda, const bf16_t* __restrict__ b, int ldb,
-                                         int rows, int cols, unsigned int* __restrict__ out) {
-    float m = 0.f;
-    const size_t total = (size_t)rows * cols;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int r = (int)(i / cols), c = (int)(i % cols);
-        m = fmaxf(m, fabsf(__bfloat162float(a[(size_t)r * lda + c]) - __bfloat162float(b[(size_t)r * ldb + c])));
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0) atomicMax(out, __float_as_uint(m));
-}
 
 // Convergence tests of a speculated chunk of mean-field sweeps: `hist` holds slots 0..n_tests of one layer's variational
 // parameters ([slot][rows_cap, ld]); flags[j] = max(flags[j], max |slot j+1 - slot j|) over the [rows, cols] window.
@@ -196,60 +182,48 @@ __global__ void ais_fused_step_kernel(double* __restrict__ logw, float a, float 
 struct DbmTC : Dbm<float> {
     std::vector<int> ldn;                        // leading dimension of a bf16 activation of layer idx (0 = visible)
     std::vector<DevBuf<bf16_t>> Wb;              // bf16 shadows of W_i: [size(i), ldn[i+1]]
-    // The layer-wise conditional adds y W_{i+1}^T to x W_i in one accumulator.  Default: a second, TRANSPOSED shadow of
-    // W_{i+1} ([H_{i+1}, ld(H_i)]) so that both operand pairs read their B operand MN-major -- the layout combination the RBM
-    // program runs.  BM_DBM_TC_MIXED=1: no second shadow, pair 1 reads W_{i+1} K-major (one op, two B layouts: saves the
-    // transposes and the memory once that op shape has been verified on the hardware).
+    // The layer-wise conditional adds y W_{i+1}^T to x W_i in one accumulator.  A second, TRANSPOSED shadow of W_{i+1}
+    // ([H_{i+1}, ld(H_i)], i >= 1) lets both operand pairs read their B operand MN-major -- the layout combination the RBM
+    // program runs.
     std::vector<DevBuf<bf16_t>> WbT;
-    bool mixed_layouts = false;
     DevBuf<bf16_t> Xb, recon_b, v_b, v2_b, v3_b;
-    std::vector<DevBuf<bf16_t>> mu_b, mu2_b, h_b, h2_b, h3_b;
+    std::vector<DevBuf<bf16_t>> mu_b, h_b, h2_b, h3_b;
     std::vector<DevBuf<float>> Gp;               // split-K slices of the gradient GEMMs
     bool particles_f32_stale = false;            // the bf16 particles are newer than the fp32 copies get_param reads
-    // mean-field as persistent dataflow programs (opt-in, BM_DBM_MF_CHUNK = sweeps per launch): slot history + programs
-    int mf_chunk = 0;
+    // mean-field as persistent dataflow programs of up to MF_CHUNK speculated sweeps per launch: slot history + programs
+    static constexpr int MF_CHUNK = 5;
+    int mf_chunk = 0;                            // MF_CHUNK, clamped by max_mf and by TC_PROGRAM_OPS, at least 1
     std::vector<DevBuf<bf16_t>> hist;            // per layer: (mf_chunk + 2) slots of [B, ldn[i+1]]
     DevBuf<unsigned int> mf_flags;
     std::map<std::pair<int, int>, std::unique_ptr<TcProgram>> mf_progs;      // keyed by (rows, sweeps in the chunk)
-    // committed particle sweeps as ONE persistent program (opt-in, BM_DBM_PCD_PROGRAM=1): keyed by (sweeps, sampled, t0)
-    bool pcd_program = false;
+    // committed particle sweeps as ONE persistent program: keyed by (sweeps, sampled, t0)
     std::map<std::tuple<int, int, int>, std::unique_ptr<TcProgram>> pcd_progs;
 
     static bool supports(const bm_dbm_cfg& f) {
         if (f.dtype != BM_DTYPE_F32) return false;
         if (!(f.v_kind == BM_UNIT_BERNOULLI || f.v_kind == BM_UNIT_GAUSSIAN)) return false;
         for (int i = 0; i < f.n_layers; ++i) if (f.h_kinds[i] != BM_UNIT_BERNOULLI) return false;
-        return true;
+        return f.n_layers <= TC_PROGRAM_OPS;     // one mean-field sweep (L ops) fits in one program
     }
 
     DbmTC(Ctx* c, const bm_dbm_cfg& f) : Dbm<float>(c, f) {
         ldn.push_back(dbm_round_up(V, 64));
         for (int i = 0; i < L; ++i) ldn.push_back(dbm_round_up(Hs[i], 64));
-        Wb.resize(L); mu_b.resize(L); mu2_b.resize(L); h_b.resize(L); h2_b.resize(L); h3_b.resize(L); Gp.resize(L);
+        Wb.resize(L); WbT.resize(L); mu_b.resize(L); h_b.resize(L); h2_b.resize(L); h3_b.resize(L); Gp.resize(L);
         Xb.ensure((size_t)B * ldn[0]); recon_b.ensure((size_t)B * ldn[0]);
         v_b.ensure((size_t)M * ldn[0]); v2_b.ensure((size_t)M * ldn[0]);
         for (DevBuf<bf16_t>* b : {&Xb, &recon_b, &v_b, &v2_b}) b->zero(ctx->stream);
         for (int i = 0; i < L; ++i) {
             Wb[i].ensure((size_t)size_of(i, V, Hs) * ldn[i + 1]);
-            mu_b[i].ensure((size_t)B * ldn[i + 1]); mu2_b[i].ensure((size_t)B * ldn[i + 1]);
+            mu_b[i].ensure((size_t)B * ldn[i + 1]);
             h_b[i].ensure((size_t)M * ldn[i + 1]); h2_b[i].ensure((size_t)M * ldn[i + 1]);
-            for (DevBuf<bf16_t>* b : {&Wb[i], &mu_b[i], &mu2_b[i], &h_b[i], &h2_b[i]}) b->zero(ctx->stream);
+            for (DevBuf<bf16_t>* b : {&Wb[i], &mu_b[i], &h_b[i], &h2_b[i]}) b->zero(ctx->stream);
         }
-        // default: persistent dataflow programs -- 5 speculated mean-field sweeps per launch, the committed particle sweeps
-        // as one launch; = 0: one launch per op
-        { const char* e = getenv("BM_DBM_MF_CHUNK"); mf_chunk = e ? atoi(e) : 5; }
-        { const char* e = getenv("BM_DBM_PCD_PROGRAM"); pcd_program = e ? atoi(e) != 0 : true; }
-        { const char* e = getenv("BM_DBM_TC_MIXED"); mixed_layouts = e && atoi(e) != 0; }
-        WbT.resize(L);
-        if (!mixed_layouts)
-            for (int i = 1; i < L; ++i) { WbT[i].ensure((size_t)Hs[i] * ldn[i]); WbT[i].zero(ctx->stream); }
-        if (mf_chunk > max_mf) mf_chunk = max_mf;
-        if (mf_chunk * L > 90) mf_chunk = 90 / L;              // a program holds at most 96 ops
-        if (mf_chunk > 0) {
-            hist.resize(L);
-            for (int i = 0; i < L; ++i) { hist[i].ensure((size_t)(mf_chunk + 2) * B * ldn[i + 1]); hist[i].zero(ctx->stream); }
-            mf_flags.ensure(mf_chunk);
-        }
+        for (int i = 1; i < L; ++i) { WbT[i].ensure((size_t)Hs[i] * ldn[i]); WbT[i].zero(ctx->stream); }
+        mf_chunk = std::max(1, std::min(std::min(MF_CHUNK, max_mf), TC_PROGRAM_OPS / L));
+        hist.resize(L);
+        for (int i = 0; i < L; ++i) { hist[i].ensure((size_t)(mf_chunk + 2) * B * ldn[i + 1]); hist[i].zero(ctx->stream); }
+        mf_flags.ensure(mf_chunk);
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
     }
 
@@ -259,7 +233,7 @@ struct DbmTC : Dbm<float> {
     void refresh_shadow(int i) {
         const int in = size_of(i, V, Hs);
         launch_f32_to_bf16(ctx, W[i].p, Hs[i], Wb[i].p, ldn[i + 1], in, Hs[i]);
-        if (i >= 1 && !mixed_layouts) {
+        if (i >= 1) {
             transpose_f32_to_bf16_kernel<<<dim3((Hs[i] + 31) / 32, (in + 31) / 32), dim3(32, 8), 0, ctx->stream>>>(W[i].p, in, Hs[i], WbT[i].p, ldn[i]);
             count_launch(ctx);
         }
@@ -269,8 +243,7 @@ struct DbmTC : Dbm<float> {
         const int H = Hs[i], Hn = Hs[i + 1];
         g.n_pairs = 2;
         g.A[1] = mat(above, rows, Hn, ldn[i + 2]); g.K[1] = Hn;
-        if (mixed_layouts) { g.B[1] = mat(Wb[i + 1].p, H, Hn, ldn[i + 2]); g.b_t[1] = false; }     // W_{i+1} stored [N, K]
-        else { g.B[1] = mat(WbT[i + 1].p, Hn, H, ldn[i + 1]); g.b_t[1] = true; }                    // W_{i+1}^T stored [K, N]
+        g.B[1] = mat(WbT[i + 1].p, Hn, H, ldn[i + 1]); g.b_t[1] = true;                              // W_{i+1}^T stored [K, N]
     }
     void narrow_state() {          // fp32 variables (as set by the caller / initialised) -> bf16 operands
         launch_f32_to_bf16(ctx, v.p, V, v_b.p, ldn[0], M, V);
@@ -376,8 +349,6 @@ struct DbmTC : Dbm<float> {
     }
 
     // ---- E-step (dbm.py:429-478) ------------------------------------------------------------------------------
-    int mean_field_tc(int rows) { return mf_chunk > 0 ? mean_field_programs(rows) : mean_field_launches(rows); }
-
     // The E-step as persistent dataflow programs: `mf_chunk` sweeps (mf_chunk x L two-pair ops) per launch, every op
     // waiting per 256-row block on the ops it reads (layer i-1 of the same sweep, layer i+1 of the previous one) --
     // no kernel boundary and no host round trip between dependent sweeps.  The sweeps of a chunk are SPECULATED: every
@@ -385,7 +356,7 @@ struct DbmTC : Dbm<float> {
     // and the host picks the first sweep index that passed, so the result and n_mf_updates are those of the
     // sweep-by-sweep loop.  Slots: 0 = S_{a-1}, 1 = S_a, 2.. = S_{a+1}...; test t of the chunk compares slots t+1 and t.
     bf16_t* slot(int i, int s) { return hist[i].p + (size_t)s * B * ldn[i + 1]; }
-    int mean_field_programs(int rows) {
+    int mean_field_tc(int rows) {
         for (int i = 0; i < L; ++i) {                                        // approximate-inference pass -> slot 0
             const bf16_t* below = i == 0 ? Xb.p : slot(i - 1, 0);
             const float sc = (i == 0 || i < L - 1) ? 2.f : 1.f;
@@ -419,7 +390,7 @@ struct DbmTC : Dbm<float> {
                 count_launch(ctx);
             }
             allreduce_max_u32(ctx, mf_flags.p, (size_t)c);       // sharded rows: the same sweep index on every rank
-            unsigned int bits[96];
+            unsigned int bits[MF_CHUNK];
             BM_CUDA(cudaMemcpyAsync(bits, mf_flags.p, (size_t)c * sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
             BM_CUDA(cudaStreamSynchronize(ctx->stream));
             int t = 0;
@@ -439,41 +410,8 @@ struct DbmTC : Dbm<float> {
         }
         for (int i = 0; i < L; ++i)
             BM_CUDA(cudaMemcpyAsync(mu_b[i].p, slot(i, result_slot), (size_t)rows * ldn[i + 1] * sizeof(bf16_t), cudaMemcpyDeviceToDevice, ctx->stream));
-        widen_mu(rows);
-        return a;
-    }
-
-    int mean_field_launches(int rows) {
-        for (int i = 0; i < L; ++i) {
-            const bf16_t* below = i == 0 ? Xb.p : mu2_b[i - 1].p;
-            const float sc = (i == 0 || i < L - 1) ? 2.f : 1.f;              // :438, :441-442
-            hidden_tc(i, below, nullptr, mu2_b[i].p, false, rows, sc, 1.f, RngKey{});
-        }
-        std::vector<bf16_t*> cur(L), nxt(L);
-        for (int i = 0; i < L; ++i) { cur[i] = mu_b[i].p; nxt[i] = mu2_b[i].p; }
-        int step = 0;
-        while (step < max_mf) {
-            BM_CUDA(cudaMemsetAsync(flag.p, 0, sizeof(unsigned int), ctx->stream));
-            for (int i = 0; i < L; ++i) {
-                max_abs_diff_bf16_kernel<<<ctx->sm_count, 256, 0, ctx->stream>>>(cur[i], ldn[i + 1], nxt[i], ldn[i + 1], rows, Hs[i], flag.p);
-                count_launch(ctx);
-            }
-            allreduce_max_u32(ctx, flag.p, 1);
-            unsigned int bits = 0;
-            BM_CUDA(cudaMemcpyAsync(&bits, flag.p, sizeof(bits), cudaMemcpyDeviceToHost, ctx->stream));
-            BM_CUDA(cudaStreamSynchronize(ctx->stream));
-            float diff; memcpy(&diff, &bits, sizeof(diff));
-            if (!(diff > (float)mf_tol)) break;                               // :451-452
-            std::vector<const bf16_t*> Hin(cur.begin(), cur.end());
-            gibbs_tc(Xb.p, Hin, nxt, nullptr, false, false, rows, 0, 0, 0);
-            std::swap(cur, nxt);                                              // :457
-            ++step;
-        }
-        for (int i = 0; i < L; ++i)
-            if (cur[i] != mu_b[i].p)
-                BM_CUDA(cudaMemcpyAsync(mu_b[i].p, cur[i], (size_t)rows * ldn[i + 1] * sizeof(bf16_t), cudaMemcpyDeviceToDevice, ctx->stream));
         widen_mu(rows);                        // get_param('mu'), transform and the bound read the fp32 variables
-        return step;
+        return a;
     }
 
     // ---- PCD particle update (dbm.py:480-509) -----------------------------------------------------------------
@@ -522,8 +460,10 @@ struct DbmTC : Dbm<float> {
         particles_f32_stale = true;
     }
 
+    // committed sweeps that fit in one program run as that program; uncommitted runs (the second half of sample_v) and
+    // longer chains take one launch per op
     void particles_tc(int n_steps, bool sample, uint64_t seed, uint32_t tick, int t0, bool commit, bf16_t** v_final) {
-        if (pcd_program && commit && n_steps >= 1 && n_steps * (L + 1) <= 90) {
+        if (commit && n_steps >= 1 && n_steps * (L + 1) <= TC_PROGRAM_OPS) {
             particles_program(n_steps, sample, seed, tick, t0);
             if (v_final) *v_final = v_b.p;
             return;
@@ -693,9 +633,8 @@ struct DbmTC : Dbm<float> {
     // (145 MB per step at 20 000 runs) never exist; up to 30 steps run as one persistent dataflow launch, every op waiting
     // per 256-run block on the op(s) it reads.  dbm.py:650-736; same draws (sites, ticks, rows) as the kernel-per-pass variant.
     void ais_local(int R, uint32_t row0, int n_betas, int k, uint64_t seed, double* logw_out) override {
-        bool epi = sample_h[0];                 // the transition's epilogue takes the linear term from sampled states
-        { const char* e = getenv("BM_DBM_AIS_EPILOGUE"); if (e && !atoi(e)) epi = false; }
-        if (!epi) { ais_local_passes(R, row0, n_betas, k, seed, logw_out); return; }
+        // the transition's epilogue takes the linear term from sampled states
+        if (!sample_h[0]) { ais_local_passes(R, row0, n_betas, k, seed, logw_out); return; }
         const int H0 = Hs[0], H1 = Hs[1];
         const int ld0 = ldn[1], ldv = ldn[0], ld1 = ldn[2];
         DevBuf<bf16_t> x, xn, va, hc;
@@ -763,14 +702,11 @@ struct DbmTC : Dbm<float> {
         }
         unit_op(true, xc, inc_a(nT - 1), inc_b(nT - 1), true, 0.f, false, 0);      // + log p_M(x_M) - log p_{M-1}(x_M)   :728
         unit_op(false, xc, inc_a(nT - 1), inc_b(nT - 1), true, 0.f, false, 0);
-        // launches of up to AIS_OPS ops; a dependency on an op of an earlier launch is the kernel boundary
-        int per = 90;
-        { const char* e = getenv("BM_DBM_AIS_OPS"); if (e && atoi(e) >= 1 && atoi(e) <= 96) per = atoi(e); }
+        // launches of up to TC_PROGRAM_OPS ops; a dependency on an op of an earlier launch is the kernel boundary
         TcProgram prog;
-        for (size_t lo = 0; lo < all.size(); lo += (size_t)per) {
-            const size_t hi = std::min(all.size(), lo + (size_t)per);
+        for (size_t lo = 0; lo < all.size(); lo += (size_t)TC_PROGRAM_OPS) {
+            const size_t hi = std::min(all.size(), lo + (size_t)TC_PROGRAM_OPS);
             prog.ops.assign(all.begin() + lo, all.begin() + hi);
-            if (getenv("BM_DEBUG_AIS")) fprintf(stderr, "ais launch: ops [%zu, %zu) of %zu, per %d\n", lo, hi, all.size(), per);
             for (size_t i = lo; i < hi; ++i) {
                 TcGemm& g = prog.ops[i - lo];
                 g.n_deps = 0;
@@ -783,8 +719,8 @@ struct DbmTC : Dbm<float> {
         BM_CUDA(cudaStreamSynchronize(ctx->stream));            // the workspaces above are released on return
     }
 
-    // the same ladder with one kernel per pass over fp32 pre-activations (BM_DBM_AIS_EPILOGUE=0; models whose first
-    // hidden layer is not sampled)
+    // the same ladder for models whose first hidden layer is not sampled: fp32 pre-activations in memory and, per temperature,
+    // one pass over them for the weight increment and the next transition's first unit updates
     void ais_local_passes(int R, uint32_t row0, int n_betas, int k, uint64_t seed, double* logw_out) {
         const int H0 = Hs[0], H1 = Hs[1];
         const int ld0 = ldn[1], ldv = ldn[0], ld1 = ldn[2];
@@ -799,21 +735,14 @@ struct DbmTC : Dbm<float> {
             linear_tc(xs, ld0, R, H0, Wb[0].p, V, H0, ld0, false, V, vb.p, pa.p);
             linear_tc(xs, ld0, R, H0, Wb[1].p, H0, H1, ld1, true, H1, hb[1].p, pb.p);
         };
-        auto accum2 = [&](const bf16_t* xs, float a, float b) {
-            ais_accum2_bf16_kernel<<<rgrid, rblock, 0, ctx->stream>>>(logw.p, a, b, xs, ld0, H0, hb[0].p, pa.p, V, pb.p, H1, R);
-            count_launch(ctx);
-        };
         bf16_t* xc = x.p; bf16_t* xo = xn.p;
         int it = 0;
-        // BM_DBM_AIS_FUSED=0: weight increment and unit updates as three separate passes over pa / pb
-        bool fused = true;
-        { const char* e = getenv("BM_DBM_AIS_FUSED"); if (e && !atoi(e)) fused = false; }
-        // `units_done`: the fused pass of this temperature step has already produced va / hc of sweep 0
-        auto transition = [&](float beta, bool have_pre, bool units_done) {
+        // `fused`: pa / pb of sweep 0 are current and the fused pass of this temperature step has already produced its va / hc
+        auto transition = [&](float beta, bool fused) {
             for (int s = 0; s < k; ++s) {
                 const uint32_t tick = (uint32_t)(it * k + s);
-                if (!(have_pre && s == 0)) pre(xc);
-                if (!(units_done && s == 0)) {
+                if (!(fused && s == 0)) {
+                    pre(xc);
                     dim3 gv(((V + 3) / 4 + 127) / 128, R), gh(((H1 + 3) / 4 + 127) / 128, R);
                     ais_unit_bf16_kernel<<<gv, 128, 0, ctx->stream>>>(pa.p, V, beta, va.p, ldv, R, V, sample_vis, make_rng(seed, SITE_AIS_V, 0, tick, row0));
                     ais_unit_bf16_kernel<<<gh, 128, 0, ctx->stream>>>(pb.p, H1, beta, hc.p, ld1, R, H1, sample_h[1], make_rng(seed, SITE_AIS_H2, 0, tick, row0));
@@ -837,9 +766,8 @@ struct DbmTC : Dbm<float> {
             ais_unit_bf16_kernel<<<g, 128, 0, ctx->stream>>>(nullptr, 0, 0.f, xc, ld0, R, H0, 1, make_rng(seed, SITE_AIS_INIT, 0, 0, row0));
             count_launch(ctx);
         }
-        // increment of the log-weights on the current x (pa / pb current) and, fused, sweep 0's unit updates at beta_next
+        // increment of the log-weights on the current x (pa / pb current) and, in the same pass, sweep 0's unit updates at beta_next
         auto step = [&](float prev, float beta, float beta_next) {
-            if (!fused) { accum2(xc, prev, beta); return; }
             const uint32_t tick = (uint32_t)(it * k);            // sweep 0 of the transition that follows
             ais_fused_step_kernel<<<rgrid, rblock, 0, ctx->stream>>>(
                 logw.p, prev, beta, beta_next, 1, xc, ld0, H0, hb[0].p,
@@ -848,17 +776,19 @@ struct DbmTC : Dbm<float> {
             count_launch(ctx);
         };
         const float delta = (float)(1.0 / n_betas);
-        transition(delta, false, false);                        // x_1 ~ T_1(x_1 | x_0)            :705
+        transition(delta, false);                               // x_1 ~ T_1(x_1 | x_0)            :705
         pre(xc);
         float beta = delta, prev = 0.f;                         // - log p_0(x_1) pairs with + log p_1(x_1) :708
         while (beta < 1.f - delta + 1e-5f) {                    // :710-711 (beta accumulates in the storage dtype)
             step(prev, beta, beta + delta);                     // + log p_i(x_i) - log p_{i-1}(x_i)  [+ v, h2 of T_{i+1}]
-            transition(beta + delta, true, fused);              // x_{i+1} ~ T_{i+1}
+            transition(beta + delta, true);                     // x_{i+1} ~ T_{i+1}
             pre(xc);
             prev = beta;
             beta = beta + delta;
         }
-        accum2(xc, prev, 1.0f);                                 // + log p_M(x_M) - log p_{M-1}(x_M)   :728
+        // + log p_M(x_M) - log p_{M-1}(x_M)   :728  (the weight-only kernel: the fused one with emit = 0 sums in another order)
+        ais_accum2_bf16_kernel<<<rgrid, rblock, 0, ctx->stream>>>(logw.p, prev, 1.0f, xc, ld0, H0, hb[0].p, pa.p, V, pb.p, H1, R);
+        count_launch(ctx);
         BM_CUDA(cudaStreamSynchronize(ctx->stream));            // the workspaces above are released on return
     }
 };

@@ -36,7 +36,6 @@ struct RbmTC : RbmSimt<float> {
     std::map<std::tuple<int, int, int, int>, std::unique_ptr<TcProgram>> progs;
     int dw_splits = 1, v_splits = 1;
     std::vector<bm_tc_op_plan> last_plan;          // the ops of the last run_program, all its launches (bm_rbm_debug_tc_plan)
-    static constexpr int PROGRAM_OPS = 90;      // ops per launch (the kernel's descriptor table holds 96)
     PeerExchange peer;             // data parallelism over NVLink peer memory (inactive on one rank / without peer access)
     // The batch buffers (X, v_k) carry two constant columns behind their V data columns -- (1, 0) for X, (1, 1) for v_k --
     // so that the dW GEMMs, run over V + 2 rows, also deliver sum(h0 - h_k) (row V) and -sum(h_k) (row V + 1): the
@@ -303,7 +302,7 @@ struct RbmTC : RbmSimt<float> {
                 if (pos_cycles > 0.8 * chain_cycles) pos_splits = 0;
             }
             { const char* e = getenv("BM_TC_DW_OVERLAP"); if (e && !atoi(e)) pos_splits = 0; }
-            if ((int)ops.size() + 4 > PROGRAM_OPS) pos_splits = 0;      // a chain cut into several launches keeps its statistics at the end
+            if ((int)ops.size() + 4 > TC_PROGRAM_OPS) pos_splits = 0;      // a chain cut into several launches keeps its statistics at the end
             const int last_v = (int)ops.size() - 2, last_h = (int)ops.size() - 1;
             if (pos_splits > 0) {
                 const int neg_splits = std::max(1, std::min(total_pairs / pair_tiles, row_chunks));
@@ -361,16 +360,16 @@ struct RbmTC : RbmSimt<float> {
                 ops.push_back(g);
             }
         }
-        if ((int)ops.size() <= PROGRAM_OPS) {
+        if ((int)ops.size() <= TC_PROGRAM_OPS) {
             if (!ops.empty()) launch_tc_program(ctx, prog, make_rng(seed, 0, 0, tick, row0), resident ? X_row0 : 0, &last_plan);
         } else {
             // a chain longer than one program holds (CD-k with 2k + 3 > 96 ops; the reference has no such limit,
-            // base_rbm.py:386-405): consecutive launches of up to PROGRAM_OPS ops -- a dependency on an op of an earlier launch is
+            // base_rbm.py:386-405): consecutive launches of up to TC_PROGRAM_OPS ops -- a dependency on an op of an earlier launch is
             // the kernel boundary
             const std::vector<TcGemm> all = ops;
             ops.clear();                         // (the cached whole-chain program object only keeps the plan)
-            for (size_t lo = 0, c = 1; lo < all.size(); lo += (size_t)PROGRAM_OPS, ++c) {
-                const size_t hi = std::min(all.size(), lo + (size_t)PROGRAM_OPS);
+            for (size_t lo = 0, c = 1; lo < all.size(); lo += (size_t)TC_PROGRAM_OPS, ++c) {
+                const size_t hi = std::min(all.size(), lo + (size_t)TC_PROGRAM_OPS);
                 std::unique_ptr<TcProgram>& part = progs[std::make_tuple(rows, k, (with_dw ? 1 : 0) | (int)(c << 1), X_mode)];
                 if (!part) part.reset(new TcProgram());
                 part->ops.assign(all.begin() + lo, all.begin() + hi);
@@ -556,10 +555,7 @@ extern "C" int bm_debug_tc_gemm(bm_ctx* hctx, int32_t M, int32_t N, int32_t K, c
     for (int i = 0; i < 2 * g.n_pairs; ++i) {
         const int pr = i / 2; const bool isA = (i % 2) == 0;
         const int Kp = pr ? K2 : K;
-        bool t = isA ? (a_t != 0) : (b_t != 0);
-        // BM_TC_DEBUG_BT2=0|1: the SECOND pair's B orientation, so that a two-pair op with mixed B layouts -- the DBM's
-        // x W_i + y W_{i+1}^T -- can be exercised through this hook (B2 is then given in that layout)
-        if (!isA && pr == 1) { const char* e = getenv("BM_TC_DEBUG_BT2"); if (e) t = atoi(e) != 0; }
+        const bool t = isA ? (a_t != 0) : (b_t != 0);
         const int mn = isA ? M : N;
         const int rows = t ? Kp : mn, cols = t ? mn : Kp;
         const int ld = round_up(cols, 8);

@@ -77,6 +77,8 @@ int tc_plan_units(Ctx* ctx, const TcGemm& g);
 // (op, row-block pair, column block) units in order; a unit starts as soon as the row blocks it reads
 // are complete (per-row-block counters in global memory), so the epilogue of one half-step overlaps
 // the MMAs of the next and no kernel boundary separates the 2k+1 GEMMs of a CD-k chain and its dW.
+// Ops the engines put into one program launch (the kernel's descriptor table holds 96); longer work goes in several launches.
+constexpr int TC_PROGRAM_OPS = 90;
 struct TcProgram {
     std::vector<TcGemm> ops;
     // device-side cache (owned by the program): descriptors + counters

@@ -160,7 +160,7 @@ typedef struct bm_dbm_cfg {
     int32_t v_kind;                  /* BM_UNIT_*                                          */
     const int32_t* h_kinds;
     const double*  h_n_samples;      /* MultinomialLayer.n_samples per layer (nullable)    */
-    int32_t dtype, compute;          /* BM_COMPUTE_BF16: tensor-core engine (F32 models, Bernoulli hidden layers); opt-in */
+    int32_t dtype, compute;          /* BM_COMPUTE_BF16: tensor-core engine (F32 models, Bernoulli hidden layers) */
     int32_t n_particles, batch_size, max_mf_updates;
     int32_t sample_v;
     const int32_t* sample_h;

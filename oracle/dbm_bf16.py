@@ -113,14 +113,29 @@ class OracleDBMbf16(OracleDBM):
             mu_new.append(self._hidden(i, below, None, False, 0, 0, 0, 0, acc_scale=sc))
         step = 0
         tol = np.float32(self.cfg.get('mf_tol', 1e-7))
-        while step < int(self.cfg.get('max_mf_updates', 10)) and \
-                max(np.max(np.abs(a - b)) for a, b in zip(mu, mu_new)) > tol:
+        self.mf_diffs = []                  # the change every convergence test of this E-step measured
+        while step < int(self.cfg.get('max_mf_updates', 10)):
+            self.mf_diffs.append(max(np.max(np.abs(a - b)) for a, b in zip(mu, mu_new)))
+            if not self.mf_diffs[-1] > tol:
+                break
             _, Hn = self.gibbs_step(Xb, mu, update_v=False, sample=False, seed=0, t=0, tick=0)
             mu, mu_new = Hn, mu
             step += 1
         for i in range(L):
             self.p['mu' + self._sfx(i)][:rows] = mu[i]
         return step
+
+    def mf_tol_stopping_at(self, X, stop):
+        """An mf_tol under which the E-step on X from the current state stops after exactly `stop` sweeps, halfway (on a log
+        scale) between the change it tests after `stop` sweeps and the smallest change before; None if there is no such gap."""
+        import copy
+        probe = copy.deepcopy(self)
+        probe.cfg.update(mf_tol=-1.0, max_mf_updates=stop + 1)
+        probe.mean_field(X)
+        d = [float(x) for x in probe.mf_diffs]
+        if not (0 < d[stop] < min(d[:stop] or [np.inf])):
+            return None
+        return float(np.sqrt(d[stop] * min(d[:stop]))) if stop else 2 * d[0]
 
     def reconstruction(self, rows):
         return self._visible(self.p['mu'][:rows], False, 0, 0, 0, 0)

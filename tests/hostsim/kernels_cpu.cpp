@@ -728,14 +728,6 @@ template <typename T> static void k_ais_unit(void** a) {
 }
 
 // ---- bm_dbm_tc.cuh ----------------------------------------------------------------------------------------------------------
-static void k_max_abs_diff_bf16(void** a) {
-    const __nv_bfloat16* x = arg<const __nv_bfloat16*>(a, 0); const int lda = arg<int>(a, 1); const __nv_bfloat16* y = arg<const __nv_bfloat16*>(a, 2);
-    const int ldb = arg<int>(a, 3), rows = arg<int>(a, 4), cols = arg<int>(a, 5); unsigned* out = arg<unsigned*>(a, 6);
-    float m = 0.f;
-    for (int r = 0; r < rows; ++r) for (int c = 0; c < cols; ++c) m = fmaxf(m, fabsf(bf2f(x[(size_t)r * lda + c]) - bf2f(y[(size_t)r * ldb + c])));
-    unsigned bits; memcpy(&bits, &m, 4);
-    if (bits > *out) *out = bits;
-}
 static void k_mf_chunk_diffs(void** a, dim3 grid) {
     const __nv_bfloat16* hist = arg<const __nv_bfloat16*>(a, 0); const size_t stride = arg<size_t>(a, 1); const int ld = arg<int>(a, 2);
     const int rows = arg<int>(a, 3), cols = arg<int>(a, 4); unsigned* flags = arg<unsigned*>(a, 5);
@@ -852,7 +844,6 @@ bool execute(const std::string& name, dim3 grid, dim3, void** args) {
     BOTH(k_dbm_bound_rows, "dbm_bound_rows_kernel", args);
     BOTH(k_ais_accum, "ais_accum_kernel", args);
     BOTH(k_ais_unit, "ais_unit_kernel", args);
-    if (has("max_abs_diff_bf16_kernel")) { k_max_abs_diff_bf16(args); return true; }
     if (has("mf_chunk_diffs_kernel")) { k_mf_chunk_diffs(args, grid); return true; }
     if (has("dbm_grad_combine_kernel")) { k_dbm_grad_combine(args); return true; }
     if (has("ais_unit_bf16_kernel")) { k_ais_unit_bf16(args); return true; }

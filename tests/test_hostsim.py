@@ -99,15 +99,9 @@ DBM_SHAPES = [(784, (512, 1024), 1024, 1024, 25), (30, (18, 11), 10, 12, 6), (30
 
 
 @pytest.mark.parametrize('V,Hs,B,M,max_mf', DBM_SHAPES)
-@pytest.mark.parametrize('mode', ['fp32', 'bf16', 'bf16-programs'])
-def test_dbm_entry_points(sim, monkeypatch, V, Hs, B, M, max_mf, mode):
+@pytest.mark.parametrize('compute', ['fp32', 'bf16'])
+def test_dbm_entry_points(sim, V, Hs, B, M, max_mf, compute):
     from boltzmann_machines import _native
-    compute = 'fp32' if mode == 'fp32' else 'bf16'
-    monkeypatch.setenv('BM_DBM_MF_CHUNK', '0')
-    monkeypatch.setenv('BM_DBM_PCD_PROGRAM', '0')
-    if mode == 'bf16-programs':
-        monkeypatch.setenv('BM_DBM_MF_CHUNK', '4')
-        monkeypatch.setenv('BM_DBM_PCD_PROGRAM', '1')
     gaussian = (V == 130)
     cfg = dbm_cfg(V, Hs, B, M, compute, gaussian, max_mf)
     rng = np.random.RandomState(1)
@@ -139,7 +133,7 @@ def test_dbm_entry_points(sim, monkeypatch, V, Hs, B, M, max_mf, mode):
     eng.get_params()
     clean(sim)
     n_prog = sim.fakecuda_launches(b'tc_program_kernel')
-    if mode == 'fp32':
+    if compute == 'fp32':
         assert n_prog == 0
     else:
         assert n_prog > 0
@@ -178,11 +172,7 @@ def executing(sim):
     sim.fakecuda_set_execute(0)
 
 
-def tc_pair(cfg, scale=0.3, seed=0):
-    from boltzmann_machines import _native
-    from oracle.dbm_bf16 import OracleDBMbf16
-    eng, emu = _native.CudaDBM(cfg), OracleDBMbf16(cfg)
-    assert eng.compute == 'bf16'
+def tc_params(cfg, scale=0.3, seed=0):
     rng = np.random.RandomState(seed)
     sizes = [cfg['n_visible']] + cfg['n_hiddens']
     d = {'vb': (0.1 * rng.randn(sizes[0])).astype(np.float32)}
@@ -190,6 +180,15 @@ def tc_pair(cfg, scale=0.3, seed=0):
         s = '' if i == 0 else '_%d' % i
         d['W' + s] = (scale * rng.randn(sizes[i], sizes[i + 1])).astype(np.float32)
         d['hb' + s] = (0.1 * rng.randn(sizes[i + 1])).astype(np.float32)
+    return d
+
+
+def tc_pair(cfg, scale=0.3, seed=0):
+    from boltzmann_machines import _native
+    from oracle.dbm_bf16 import OracleDBMbf16
+    eng, emu = _native.CudaDBM(cfg), OracleDBMbf16(cfg)
+    assert eng.compute == 'bf16'
+    d = tc_params(cfg, scale, seed)
     for e in (eng, emu):
         e.set_params(d)
         e.init_particles(4242)
@@ -211,15 +210,7 @@ def no_skips(sim):
 
 
 @pytest.mark.parametrize('Hs', [(18,), (18, 11), (18, 11, 7), (70, 130)])
-@pytest.mark.parametrize('programs', [False, True])
-@pytest.mark.parametrize('mixed', ['0', '1'])
-def test_tc_dbm_queries_equal_the_bf16_emulation(executing, monkeypatch, Hs, programs, mixed):
-    monkeypatch.setenv('BM_DBM_TC_MIXED', mixed)        # 0: transposed second shadow (default); 1: one op, two B layouts
-    monkeypatch.setenv('BM_DBM_MF_CHUNK', '0')
-    monkeypatch.setenv('BM_DBM_PCD_PROGRAM', '0')
-    if programs:
-        monkeypatch.setenv('BM_DBM_MF_CHUNK', '4')
-        monkeypatch.setenv('BM_DBM_PCD_PROGRAM', '1')
+def test_tc_dbm_queries_equal_the_bf16_emulation(executing, Hs):
     cfg = small_cfg(Hs)
     eng, emu = tc_pair(cfg)
     g, w = eng.get_params(), emu.get_params()
@@ -243,15 +234,7 @@ def test_tc_dbm_queries_equal_the_bf16_emulation(executing, monkeypatch, Hs, pro
 
 
 @pytest.mark.parametrize('Hs,gaussian', [((18,), False), ((18, 11), False), ((18, 11, 7), False), ((18, 11), True)])
-@pytest.mark.parametrize('programs', [False, True])
-@pytest.mark.parametrize('mixed', ['0', '1'])
-def test_tc_dbm_training_steps_equal_the_bf16_emulation(executing, monkeypatch, Hs, gaussian, programs, mixed):
-    monkeypatch.setenv('BM_DBM_TC_MIXED', mixed)
-    monkeypatch.setenv('BM_DBM_MF_CHUNK', '0')
-    monkeypatch.setenv('BM_DBM_PCD_PROGRAM', '0')
-    if programs:
-        monkeypatch.setenv('BM_DBM_MF_CHUNK', '3')
-        monkeypatch.setenv('BM_DBM_PCD_PROGRAM', '1')
+def test_tc_dbm_training_steps_equal_the_bf16_emulation(executing, Hs, gaussian):
     cfg = small_cfg(Hs, gaussian=gaussian)
     eng, emu = tc_pair(cfg)
     rng = np.random.RandomState(5)
@@ -268,13 +251,44 @@ def test_tc_dbm_training_steps_equal_the_bf16_emulation(executing, monkeypatch, 
     eng.close()
 
 
-@pytest.mark.parametrize('k,fused', [(1, 'epilogue'), (3, 'epilogue'), (1, '1'), (1, '0'), (3, '1')])
-@pytest.mark.parametrize('mixed', ['0', '1'])
-def test_tc_dbm_ais_equals_the_bf16_emulation(executing, monkeypatch, k, fused, mixed):
-    monkeypatch.setenv('BM_DBM_TC_MIXED', mixed)
-    monkeypatch.setenv('BM_DBM_AIS_EPILOGUE', '1' if fused == 'epilogue' else '0')
-    monkeypatch.setenv('BM_DBM_AIS_FUSED', '0' if fused == '0' else '1')
-    cfg = small_cfg((5, 4), V=7, n_particles=4, batch_size=4)
+@pytest.mark.parametrize('Hs,scale', [((18, 11), 0.6), ((18, 11, 7), 0.6), ((70, 130), 0.3)])
+@pytest.mark.parametrize('stop', [2, 5, 7, 'never', 'no-updates'])
+def test_tc_dbm_e_step_stops_where_the_emulation_does(executing, Hs, scale, stop):
+    """The E-step runs as programs of up to 5 speculated sweeps (DbmTC::MF_CHUNK) and keeps the first sweep whose convergence
+    test passed.  It must stop where the emulation's sweep-by-sweep loop does: inside the first program (2), at its last sweep
+    (5), in a later one (7), at max_mf_updates = 12 (never converged), and without a sweep at max_mf_updates = 0 (mu
+    unchanged).  The tolerance for a given stop is read off the emulation's own convergence measures."""
+    from oracle.dbm_bf16 import OracleDBMbf16
+    cfg = small_cfg(Hs, max_mf_updates=0 if stop == 'no-updates' else 12, mf_tol=-1.0)
+    X = (np.random.RandomState(9).rand(7, cfg['n_visible']) < 0.3).astype(np.float32)
+    if isinstance(stop, int):
+        probe = OracleDBMbf16(cfg)
+        probe.set_params(tc_params(cfg, scale))
+        probe.init_particles(4242)
+        cfg['mf_tol'] = probe.mf_tol_stopping_at(X, stop)
+        assert cfg['mf_tol'] is not None, 'no tolerance stops the emulation after %d sweeps' % stop
+    want = {'never': 12, 'no-updates': 0}.get(stop, stop)
+    eng, emu = tc_pair(cfg, scale)
+    mu0 = eng.get_params(['mu'])['mu']
+    a, b = eng.val_metrics(X, 1, 7, 3), emu.val_metrics(X, 1, 7, 3)
+    assert a['n_mf_updates'] == b['n_mf_updates'] == want, (a['n_mf_updates'], b['n_mf_updates'])
+    assert a['msre'] == pytest.approx(b['msre'], rel=1e-3)
+    g, w = eng.get_params(), emu.get_params()
+    for k in w:
+        if k.startswith('mu') and not k.startswith('mu_means'):
+            np.testing.assert_allclose(g[k], w[k], rtol=2.0 ** -7, atol=1e-6, err_msg=k)
+    if stop == 'no-updates':
+        np.testing.assert_array_equal(g['mu'], mu0)
+    no_skips(executing)
+    eng.close()
+
+
+@pytest.mark.parametrize('k', [1, 3])
+@pytest.mark.parametrize('sample_h',[[True, True], [False, True]], ids=['epilogue', 'passes'])
+def test_tc_dbm_ais_equals_the_bf16_emulation(executing, k, sample_h):
+    """A sampled first hidden layer runs the ladder in the tensor-core ops' epilogues; an unsampled one runs it over fp32
+    pre-activations in memory (DbmTC::ais_local_passes)."""
+    cfg = small_cfg((5, 4), V=7, n_particles=4, batch_size=4, sample_h=sample_h)
     eng, emu = tc_pair(cfg)
     a = eng.ais(16, 60, k, 2222)
     b = emu.ais(16, 60, k, 2222)
@@ -481,25 +495,23 @@ def test_structural_cost_of_the_hot_entry_points(sim):
     eng.close()
 
 
-def test_random_tc_dbm_configurations_equal_the_bf16_emulation(executing, monkeypatch):
-    """tools/fuzz_dbm_tc_hostsim.py over a fixed range of seeds: ragged widths, 1-3 hidden layers, Gaussian visibles, every
-    combination of the engine's switches; one training step at a time from identical states, then queries and AIS."""
+def test_random_tc_dbm_models_equal_the_bf16_emulation(executing):
+    """tools/fuzz_dbm_tc_hostsim.py over a fixed range of seeds: ragged widths, 1-3 hidden layers, Gaussian visibles, sampled
+    and mean-valued layers; one training step at a time from identical states, then queries and AIS."""
     import importlib.util
     spec = importlib.util.spec_from_file_location('fuzz_dbm_tc_hostsim', os.path.join(ROOT, 'tools', 'fuzz_dbm_tc_hostsim.py'))
     fuzz = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(fuzz)
-    for k in ('BM_DBM_TC_MIXED', 'BM_DBM_AIS_FUSED', 'BM_DBM_MF_CHUNK', 'BM_DBM_PCD_PROGRAM'):
-        monkeypatch.setenv(k, '0')                       # restored afterwards (the tool sets them per configuration)
     outcomes = {}
     for seed in range(900000, 900150):
-        cfg, env, run = fuzz.draw(np.random.RandomState(seed))
-        r = fuzz.one(cfg, env, run, seed, executing)
+        cfg, run = fuzz.draw(np.random.RandomState(seed))
+        r = fuzz.one(cfg, run, seed, executing)
         outcomes[r] = outcomes.get(r, 0) + 1
     assert outcomes.get("ok", 0) >= 145 and not outcomes.get("FAIL"), outcomes   # (mf-count, sample-flip: rounding events, see the tool)
     assert executing.fakecuda_hazard_launches() > 100          # the programs' dataflow was checked on the way
 
 
-def test_program_dataflow_hazards_are_checked_and_a_missing_dependency_is_caught(executing, monkeypatch):
+def test_program_dataflow_hazards_are_checked_and_a_missing_dependency_is_caught(executing):
     """On the GPU the units of a program run concurrently, ordered only by the dependencies the host declares; the interpreter
     runs the ops in program order, so it shadows every element a launch touches and reports reads / overwrites no dependency
     path covers (row block by row block).  Clean: the GPU-verified RBM step program and the tensor-core DBM engine's mean-field
@@ -545,13 +557,9 @@ def test_program_dataflow_hazards_are_checked_and_a_missing_dependency_is_caught
     for op in (2, 3, 4, 5, 6, 7):
         _, v = rbm_step(drop=(op, 0))
         assert 'without a dependency path' in v, (op, v)
-    monkeypatch.setenv('BM_DBM_MF_CHUNK', '3')
-    monkeypatch.setenv('BM_DBM_PCD_PROGRAM', '1')
-    for mixed in ('0', '1'):
-        monkeypatch.setenv('BM_DBM_TC_MIXED', mixed)
-        for Hs in ((40,), (40, 24), (40, 24, 16)):
-            checked, v = dbm_step(Hs)
-            assert checked >= 2 and v == '', (Hs, mixed, v)
+    for Hs in ((40,), (40, 24), (40, 24, 16)):
+        checked, v = dbm_step(Hs)
+        assert checked >= 2 and v == '', (Hs, v)
     for op in (1, 2, 3):
         _, v = dbm_step((40, 24), drop=(op, 0))
         assert 'without a dependency path' in v, (op, v)

@@ -1,8 +1,6 @@
 """Tensor-core DBM engine (compute='bf16', csrc/bm_dbm_tc.cuh) against its bf16-operand emulation
-(oracle/dbm_bf16.py), the pinned fp32 oracle and exact enumeration.
-
-Both operand-layout variants; the engine is the default for
-float32 models with Bernoulli hidden layers."""
+(oracle/dbm_bf16.py), the pinned fp32 oracle and exact enumeration.  The engine is the default for float32 models with
+Bernoulli hidden layers."""
 import os
 
 import numpy as np
@@ -65,11 +63,8 @@ def test_state_roundtrip_is_bf16_for_activations_and_fp32_for_variables():
 
 
 @pytest.mark.parametrize('Hs', [(18,), (18, 11), (18, 11, 7), (70, 130)])
-@pytest.mark.parametrize('mixed', ['0', '1'])
-def test_mean_field_and_queries(monkeypatch, Hs, mixed):
-    """mixed = 0 (default): the second operand pair reads a transposed shadow of W_{i+1}, both pairs MN-major; 1: one op with
-    two B layouts and no second shadow (BM_DBM_TC_MIXED)."""
-    monkeypatch.setenv('BM_DBM_TC_MIXED', mixed)
+def test_mean_field_and_queries(Hs):
+    """The second operand pair of a conditional reads a transposed shadow of W_{i+1}: both pairs MN-major."""
     cfg = make_cfg(Hs=Hs)
     eng, emu = _native.CudaDBM(cfg), OracleDBMbf16(cfg)
     init(cfg, (eng, emu))
@@ -122,8 +117,8 @@ _EMU_AIS = {}
 
 
 def _emulated_ladder(cfg, k, n_betas):
-    """the bf16 emulation's ladder (numpy loops: a minute per call) is the same for every engine variant: computed once"""
-    key = (k, n_betas)
+    """the bf16 emulation's ladder (numpy loops: a minute per call), computed once per model"""
+    key = (k, n_betas, tuple(cfg['sample_h']))
     if key not in _EMU_AIS:
         emu = OracleDBMbf16(cfg)
         init(cfg, (emu,))
@@ -131,13 +126,10 @@ def _emulated_ladder(cfg, k, n_betas):
     return _EMU_AIS[key]
 
 
-@pytest.mark.parametrize('variant,k', [('epilogue', 1), ('fused', 1), ('passes', 1), ('epilogue', 3), ('fused', 3), ('passes', 3)])
-def test_ais_matches_exact_enumeration(monkeypatch, variant, k):
-    """epilogue (default): weight increments and unit updates inside the epilogues of the three tensor-core ops of a temperature
-    step, up to 30 steps per persistent launch; fused (BM_DBM_AIS_EPILOGUE=0): fp32 pre-activations + one pass over them per
-    temperature; passes (also BM_DBM_AIS_FUSED=0): three passes.  Same expressions, same Philox sites."""
-    monkeypatch.setenv('BM_DBM_AIS_EPILOGUE', '1' if variant == 'epilogue' else '0')
-    monkeypatch.setenv('BM_DBM_AIS_FUSED', '0' if variant == 'passes' else '1')
+@pytest.mark.parametrize('k', [1, 3])
+def test_ais_matches_exact_enumeration(k):
+    """Weight increments and unit updates inside the epilogues of the three tensor-core ops of a temperature step, up to 30
+    steps per persistent launch (a model whose first hidden layer is sampled)."""
     cfg = make_cfg(V=7, Hs=(5, 4), n_particles=4, batch_size=4)
     n_betas = 240 if k == 1 else 120
     eng = _native.CudaDBM(cfg)
@@ -154,6 +146,22 @@ def test_ais_matches_exact_enumeration(monkeypatch, variant, k):
         terms.append(x @ p['hb'] + np.logaddexp(0, W0 @ x + p['vb']).sum() + np.logaddexp(0, x @ W1 + p['hb_1']).sum())
     exact = np.logaddexp.reduce(terms)
     assert abs(lm(a) - exact) < 0.15, (lm(a), exact)
+    eng.close()
+
+
+@pytest.mark.parametrize('k', [1, 3])
+def test_ais_of_a_mean_valued_first_layer_matches_the_emulation(k):
+    """A model whose first hidden layer is not sampled runs the ladder over fp32 pre-activations in memory, one fused pass over
+    them per temperature (DbmTC::ais_local_passes): same expressions, same Philox sites as the emulation."""
+    cfg = make_cfg(V=7, Hs=(5, 4), n_particles=4, batch_size=4, sample_h=[False, True])
+    n_betas = 240 if k == 1 else 120
+    eng = _native.CudaDBM(cfg)
+    init(cfg, (eng,))
+    a = eng.ais(32, n_betas, k, 2222)
+    b, _ = _emulated_ladder(cfg, k, n_betas)
+    lm = lambda v: np.logaddexp.reduce(v) - np.log(len(v))
+    assert abs(lm(a) - lm(b)) < 0.1
+    assert np.mean(np.abs(a - b) < 2e-3) > 0.8           # the same chains, but for a draw at rounding distance of its probability
     eng.close()
 
 
@@ -224,67 +232,63 @@ def test_cfg4_shape_step_agrees_with_the_fp32_engine():
     tc.close(); simt.close()
 
 
-@pytest.mark.parametrize('chunk', [1, 3, 6, 25])
-@pytest.mark.parametrize('Hs,rows', [((18, 11), 10), ((18, 11, 7), 10), ((512, 1024), 300)])
-def test_mean_field_programs_equal_the_sweep_by_sweep_loop(monkeypatch, chunk, Hs, rows):
-    """BM_DBM_MF_CHUNK=C runs the E-step as persistent dataflow programs of C speculated sweeps per launch; the first
-    sweep index whose convergence test passes is picked afterwards, so mu and n_mf_updates are those of the
-    launch-per-op loop up to fp32 summation order."""
+@pytest.mark.parametrize('Hs,rows,stop', [(Hs, rows, stop) for Hs, rows in (((18, 11), 10), ((18, 11, 7), 10))
+                                           for stop in (2, 5, 7, 'never', 'no-updates')] +
+                                          [((512, 1024), 300, stop) for stop in (2, 5, 'never', 'no-updates')])
+def test_mean_field_programs_equal_the_emulation(Hs, rows, stop):
+    """The E-step runs as persistent dataflow programs of up to 5 speculated sweeps per launch (DbmTC::MF_CHUNK); the first
+    sweep index whose convergence test passes is picked afterwards, so mu and n_mf_updates are those of the emulation's
+    sweep-by-sweep loop up to fp32 summation order.  Stops inside the first program (2), at its last sweep (5), in a later one
+    (7), at max_mf_updates = 8 (never converged: a second program of 3 sweeps), and at max_mf_updates = 0 (mu unchanged); the
+    tolerance for a stop is read off the emulation's convergence measures.  The 784-512-1024 model converges to a one-ulp
+    oscillation by its sixth sweep, so its later program is reached through max_mf_updates only."""
     V = 30 if Hs[0] < 100 else 784
-    cfg = make_cfg(V=V, Hs=Hs, batch_size=max(rows, 10), max_mf_updates=7, mf_tol=2e-3)
-    monkeypatch.setenv('BM_DBM_MF_CHUNK', '0')
-    loop = _native.CudaDBM(cfg)
-    monkeypatch.setenv('BM_DBM_MF_CHUNK', str(chunk))
-    prog = _native.CudaDBM(cfg)
-    init(cfg, (loop, prog), scale=0.3 if V == 30 else 0.03)
+    scale = 0.6 if V == 30 else 0.04
+    cfg = make_cfg(V=V, Hs=Hs, batch_size=max(rows, 10), max_mf_updates=0 if stop == 'no-updates' else 8, mf_tol=-1.0)
+    if isinstance(stop, int):
+        probe = OracleDBMbf16(cfg)
+        init(cfg, (probe,), scale=scale)
+        cfg['mf_tol'] = probe.mf_tol_stopping_at(batch(cfg, rows, seed=0), stop)
+        assert cfg['mf_tol'] is not None, 'no tolerance stops the emulation after %d sweeps' % stop
+    eng, emu = _native.CudaDBM(cfg), OracleDBMbf16(cfg)
+    init(cfg, (eng, emu), scale=scale)
+    mu0 = eng.get_params(['mu'])['mu']
+    names = ['mu' + ('' if i == 0 else '_%d' % i) for i in range(len(Hs))]
     for it in range(2):                      # the second E-step starts from the first one's mu (stale-mu quirk)
         X = batch(cfg, rows, seed=it)
-        a, b = loop.val_metrics(X, 1, 5, it), prog.val_metrics(X, 1, 5, it)
-        # same ops and operands; only the order in which a consumer adds its K chunks may follow the producers'
-        # completion order (granule-level dataflow), i.e. fp32 rounding before the bf16 store
+        a, b = eng.val_metrics(X, 1, 5, it), emu.val_metrics(X, 1, 5, it)
+        if it == 0:
+            assert b['n_mf_updates'] == {'never': 8, 'no-updates': 0}.get(stop, stop)
+        # only the order in which a consumer adds its K chunks may follow the producers' completion order (granule-level
+        # dataflow), i.e. fp32 rounding before the bf16 store
         assert abs(a['n_mf_updates'] - b['n_mf_updates']) <= 1
         assert a['msre'] == pytest.approx(b['msre'], rel=1e-2)
-        ga, gb = loop.get_params(), prog.get_params()
-        for k in ga:
+        ga, gb = eng.get_params(names), emu.get_params(names)
+        for k in names:
             np.testing.assert_allclose(ga[k], gb[k], rtol=2.0 ** -7, atol=1e-3, err_msg=k)
             assert np.mean(ga[k] != gb[k]) < 0.02, k
-    loop.close(); prog.close()
+    if stop == 'no-updates':
+        np.testing.assert_array_equal(ga['mu'], mu0)
+    eng.close()
 
 
 @pytest.mark.parametrize('Hs,k', [((18,), 3), ((18, 11), 1), ((18, 11, 7), 2), ((512,), 5), ((512, 256), 2)])
-def test_particle_sweep_program_equals_the_launch_per_op_sweeps(monkeypatch, Hs, k):
-    """BM_DBM_PCD_PROGRAM=1: the k committed sweeps of the persistent chains (k x (L + 1) ops) run as ONE persistent
-    dataflow program; same ops, same Philox sites -> the same particles up to draws at rounding-level ties."""
+def test_particle_sweep_program_equals_the_emulation(Hs, k):
+    """The k committed sweeps of the persistent chains (k x (L + 1) ops) run as ONE persistent dataflow program; same
+    ops, same Philox sites as the emulation -> the same particles up to draws at rounding-level ties."""
     V = 30 if Hs[0] < 100 else 784
     cfg = make_cfg(V=V, Hs=Hs, n_particles=12 if V == 30 else 300, batch_size=10)
-    monkeypatch.setenv('BM_DBM_PCD_PROGRAM', '0')
-    loop = _native.CudaDBM(cfg)
-    monkeypatch.setenv('BM_DBM_PCD_PROGRAM', '1')
-    prog = _native.CudaDBM(cfg)
-    init(cfg, (loop, prog), scale=0.3 if V == 30 else 0.03)
+    eng, emu = _native.CudaDBM(cfg), OracleDBMbf16(cfg)
+    init(cfg, (eng, emu), scale=0.3 if V == 30 else 0.03)
     X = batch(cfg, 10)
     for it in range(2):
-        loop.val_metrics(X, k, 5, it), prog.val_metrics(X, k, 5, it)
+        eng.val_metrics(X, k, 5, it), emu.val_metrics(X, k, 5, it)
         names = ['v'] + ['h' + ('' if i == 0 else '_%d' % i) for i in range(len(Hs))]
-        ga, gb = loop.get_params(names), prog.get_params(names)
+        ga, gb = eng.get_params(names), emu.get_params(names)
         for n in names:
-            assert set(np.unique(gb[n])) <= {0.0, 1.0}, n
+            assert set(np.unique(ga[n])) <= {0.0, 1.0}, n
             assert np.mean(ga[n] != gb[n]) < 0.05, (n, np.mean(ga[n] != gb[n]))
-    loop.close(); prog.close()
-
-
-@pytest.mark.parametrize('M,N,K1,K2', [(200, 512, 784, 1024), (1024, 512, 784, 1024), (33, 18, 30, 11), (300, 130, 70, 257)])
-def test_raw_two_pair_op_with_mixed_b_layouts(monkeypatch, M, N, K1, K2):
-    """The one op shape of the tensor-core DBM engine that no other test reaches at the kernel level: ONE accumulator fed by
-    pair 0 with B stored [K, N] (x W_i) and pair 1 with B stored [N, K] (y W_{i+1}^T).  Run this first on a new box."""
-    rng = np.random.RandomState(M + N)
-    A1, B1 = rng.rand(M, K1), 0.1 * rng.randn(K1, N)          # MN-major B
-    A2, B2 = rng.rand(M, K2), 0.1 * rng.randn(N, K2)          # K-major B
-    monkeypatch.setenv('BM_TC_DEBUG_BT2', '0')
-    C = _native.debug_tc_gemm(A1, B1, a_t=False, b_t=True, A2=A2, B2=B2)
-    r = lambda x: bf16_round(x).astype(np.float64)
-    want = r(A1) @ r(B1) + r(A2) @ r(B2).T
-    np.testing.assert_allclose(C, want, atol=5e-2, rtol=1e-3)
+    eng.close()
 
 
 @pytest.mark.parametrize('M,N,K1,K2', [(200, 512, 784, 1024), (1024, 512, 784, 1024), (33, 18, 30, 11), (300, 130, 70, 257)])

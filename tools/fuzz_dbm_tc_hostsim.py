@@ -1,6 +1,7 @@
 """Random configurations of the tensor-core DBM engine (compute='bf16'), its kernels interpreted on the CPU (tests/hostsim),
-against the bf16 emulation oracle (oracle/dbm_bf16.py): training steps, queries and AIS on ragged shapes, every combination of
-the engine's switches (program variants, mixed operand layouts, fused AIS step).
+against the bf16 emulation oracle (oracle/dbm_bf16.py): training steps, queries and AIS on ragged shapes, Gaussian visibles,
+sampled and mean-valued layers (an unsampled first hidden layer takes the AIS ladder over fp32 pre-activations), 1-3 hidden
+layers and now and then several 256-row blocks.
 
     python tools/fuzz_dbm_tc_hostsim.py [--n 200] [--seed 0]
 
@@ -41,13 +42,10 @@ def draw(rng):
         # several 256-row blocks: the programs' row-block dependencies are then checked block by block (the interpreter shadows
         # every element a program launch touches and reports hazards no declared dependency covers)
         cfg['batch_size'], cfg['n_particles'] = int(rng.randint(257, 700)), int(rng.randint(257, 700))
-    env = dict(BM_DBM_TC_MIXED=str(rng.randint(0, 2)), BM_DBM_AIS_FUSED=str(rng.randint(0, 2)))
-    env['BM_DBM_MF_CHUNK'] = str(rng.randint(1, 6)) if rng.rand() < 0.6 else '0'        # 0: one launch per op (the default is 5)
-    env['BM_DBM_PCD_PROGRAM'] = '1' if rng.rand() < 0.6 else '0'
     run = dict(k=int(rng.randint(1, 4)), steps=int(rng.randint(1, 4)), lr=float(rng.choice([0.01, 0.05, 0.2])),
                momentum=float(rng.choice([0., 0.5, 0.9])), scale=float(rng.choice([0.05, 0.3, 1.0])),
                rows=[int(rng.randint(1, cfg['batch_size'] + 1)) if rng.rand() < 0.3 else cfg['batch_size'] for _ in range(3)])
-    return cfg, env, run
+    return cfg, run
 
 
 def close(got, want, what, rtol=2.0 ** -7, atol=3e-5):
@@ -63,14 +61,11 @@ def close(got, want, what, rtol=2.0 ** -7, atol=3e-5):
         '{0}: {1} of {2} elements off, max |diff| {3:.3g}'.format(what, int(bad.sum()), bad.size, float(d.max()))
 
 
-def one(cfg, env, run, seed, sim=None):
+def one(cfg, run, seed, sim=None):
     """One configuration.  `sim`: the host-simulation library, whose runtime checks are then asserted too (None: the
     engine runs on a real GPU)."""
     from boltzmann_machines import _native
     from oracle.dbm_bf16 import OracleDBMbf16
-    for k in ('BM_DBM_TC_MIXED', 'BM_DBM_AIS_FUSED', 'BM_DBM_MF_CHUNK', 'BM_DBM_PCD_PROGRAM', 'BM_DBM_AIS_EPILOGUE'):
-        os.environ.pop(k, None)
-    os.environ.update(env)
     if sim is not None:
         sim.fakecuda_reset()
     eng, emu = _native.CudaDBM(cfg), OracleDBMbf16(cfg)
@@ -143,13 +138,13 @@ def main():
     sim.fakecuda_hazard_launches.restype = C.c_long
     for i in range(args.n):
         seed = args.seed * 100000 + i
-        cfg, env, run = draw(np.random.RandomState(seed))
+        cfg, run = draw(np.random.RandomState(seed))
         try:
-            r = one(cfg, env, run, seed, sim)
+            r = one(cfg, run, seed, sim)
         except Exception as e:            # noqa: BLE001 -- report and go on
             r = 'FAIL'
             msg = ' '.join(str(e).split())[:400]
-            print('FAIL seed={0} cfg={1} env={2} run={3}\n     {4}'.format(seed, {k: v for k, v in cfg.items() if k != 'sigma'}, env, run, msg),
+            print('FAIL seed={0} cfg={1} run={2}\n     {3}'.format(seed, {k: v for k, v in cfg.items() if k != 'sigma'}, run, msg),
                   flush=True)
             if not isinstance(e, AssertionError):
                 traceback.print_exc()

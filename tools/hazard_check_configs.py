@@ -6,7 +6,7 @@ Every element a program launch reads or writes is shadowed while the launch is i
 `Hazards`); a read of / write over something another op of the launch touched must be covered by a declared dependency path,
 256-row block by 256-row block.  cfg2: Bernoulli RBM 784-1024, batch 4096, CD-5 (the benchmark's program, 16 row blocks).
 cfg3: Gaussian RBM 3072-5000, batch 512 (host batch and resident-dataset step).  cfg4: the tensor-core DBM engine's mean-field
-and particle programs, 784-512-1024, batch = particles = 1024, both operand-layout variants.  About 3 minutes, 2 GB."""
+and particle programs, 784-512-1024, batch = particles = 1024.  About 3 minutes, 2 GB."""
 import ctypes as C
 import os
 import subprocess
@@ -63,21 +63,18 @@ def main():
         eng.close()
     if 'cfg4' in which:
         V, Hs, B = 784, (512, 1024), 1024
-        os.environ['BM_DBM_MF_CHUNK'], os.environ['BM_DBM_PCD_PROGRAM'] = '4', '1'
-        for mixed in ('0', '1'):
-            os.environ['BM_DBM_TC_MIXED'] = mixed
-            cfg = dict(n_visible=V, n_hiddens=list(Hs), v_kind='bernoulli', h_kinds=['bernoulli'] * 2, h_n_samples=[100.] * 2,
-                       dtype='float32', compute='bf16', n_particles=B, batch_size=B, max_mf_updates=8, mf_tol=1e-6, l2=1e-4,
-                       max_norm=3.0, sample_v=True, sample_h=[True] * 2, sparsity_target=[0.2] * 2, sparsity_cost=[0.01] * 2,
-                       sparsity_damping=0.9)
-            eng = _native.CudaDBM(cfg)
-            eng.set_params({'vb': np.zeros(V, np.float32), 'W': (0.01 * rng.randn(V, 512)).astype(np.float32),
-                            'hb': np.zeros(512, np.float32), 'W_1': (0.01 * rng.randn(512, 1024)).astype(np.float32),
-                            'hb_1': np.zeros(1024, np.float32)})
-            eng.init_particles(1)
-            eng.train_step((rng.rand(B, V) < 0.2).astype(np.float32), 0.01, 0.5, 5, 7, 0)
-            ok = report('cfg4 DBM programs (BM_DBM_TC_MIXED={0})'.format(mixed)) and ok
-            eng.close()
+        cfg = dict(n_visible=V, n_hiddens=list(Hs), v_kind='bernoulli', h_kinds=['bernoulli'] * 2, h_n_samples=[100.] * 2,
+                   dtype='float32', compute='bf16', n_particles=B, batch_size=B, max_mf_updates=8, mf_tol=1e-6, l2=1e-4,
+                   max_norm=3.0, sample_v=True, sample_h=[True] * 2, sparsity_target=[0.2] * 2, sparsity_cost=[0.01] * 2,
+                   sparsity_damping=0.9)
+        eng = _native.CudaDBM(cfg)
+        eng.set_params({'vb': np.zeros(V, np.float32), 'W': (0.01 * rng.randn(V, 512)).astype(np.float32),
+                        'hb': np.zeros(512, np.float32), 'W_1': (0.01 * rng.randn(512, 1024)).astype(np.float32),
+                        'hb_1': np.zeros(1024, np.float32)})
+        eng.init_particles(1)
+        eng.train_step((rng.rand(B, V) < 0.2).astype(np.float32), 0.01, 0.5, 5, 7, 0)
+        ok = report('cfg4 DBM programs') and ok
+        eng.close()
     sys.exit(0 if ok else 1)
 
 
