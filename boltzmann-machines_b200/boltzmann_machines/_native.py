@@ -30,7 +30,7 @@ EXPORTS = (
     'bm_rbm_get_activation', 'bm_debug_tc_gemm', 'bm_debug_tc_op', 'bm_rbm_debug_tc_plan',
     'bm_dbm_create', 'bm_dbm_destroy', 'bm_dbm_set_param', 'bm_dbm_get_param', 'bm_dbm_init_particles',
     'bm_dbm_train_step', 'bm_dbm_val_metrics', 'bm_dbm_transform', 'bm_dbm_reconstruct', 'bm_dbm_log_proba',
-    'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows',
+    'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows', 'bm_debug_dbm_multinomial_rows',
 )
 
 
@@ -143,6 +143,7 @@ def load_library(path=None):
         'bm_dbm_log_proba': [vp, vp, i32, vp], 'bm_dbm_sample_v': [vp, i32, u64, u32, vp],
         'bm_dbm_ais': [vp, i32, i32, i32, u64, vp],
         'bm_dbm_ais_rows': [vp, i32, i32, i32, u64, u32, vp],
+        'bm_debug_dbm_multinomial_rows': [vp, vp, i32, i32, dbl, i32, u64, u32, u32, u32, vp, vp, vp, vp],
     }
     for name, argtypes in protos.items():
         fn = getattr(lib, name)
@@ -417,6 +418,22 @@ def debug_tc_op(pairs, outputs=('f32',), splits=1, force_bn=0, force_cluster=0, 
     return out
 
 
+def debug_dbm_multinomial_rows(pre, n_samples, n_draws, seed, site, t, tick, ctx=None):
+    """The tensor-core DBM engine's multinomial row kernel on fp32 pre-activations (test hook,
+    bm_debug_dbm_multinomial_rows).  Returns (bf16 bit patterns, fp32 output, reference means, reference counts or None):
+    the last two from the CUDA-core engine's softmax_rows + multinomial_rows kernels on the same input."""
+    ctx = ctx or Context.default()
+    pre = np.ascontiguousarray(pre, dtype=np.float32)
+    rows, cols = pre.shape
+    out_bf = np.empty((rows, cols), np.uint16)
+    out_f32, ref_means = np.empty((rows, cols), np.float32), np.empty((rows, cols), np.float32)
+    ref_counts = np.empty((rows, cols), np.float32) if n_draws > 0 else None
+    check(load_library().bm_debug_dbm_multinomial_rows(
+        ctx.handle, pre.ctypes.data, rows, cols, float(n_samples), int(n_draws), int(seed), int(site), int(t), int(tick),
+        out_bf.ctypes.data, out_f32.ctypes.data, ref_means.ctypes.data, None if ref_counts is None else ref_counts.ctypes.data))
+    return out_bf, out_f32, ref_means, ref_counts
+
+
 def _mask(names):
     m = 0
     for n in names:
@@ -636,12 +653,16 @@ class CudaDBM(object):
         # float32 models with Bernoulli hidden layers (binary or Gaussian visibles) run on the tensor-core engine
         # (csrc/bm_dbm_tc.cuh: bf16 operands, fp32 accumulation) -- the same rule as DbmTC::supports(); compute='fp32'
         # (or BM_DBM_COMPUTE / BM_COMPUTE = fp32) selects the storage-precision CUDA-core engine, which every other
-        # model uses anyway.
+        # model uses anyway.  Multinomial hidden layers run on the tensor-core engine as well, but only when the caller asks
+        # for it by name: compute='bf16' or BM_DBM_COMPUTE=bf16 (BM_COMPUTE alone leaves them on the fp32 engine).
         compute = 'fp32'
+        h_kinds = cfg.get('h_kinds', ['bernoulli'] * self.L)
         tc_ok = (self.dt == np.float32 and cfg.get('v_kind', 'bernoulli') in ('bernoulli', 'gaussian') and
-                 all(k == 'bernoulli' for k in cfg.get('h_kinds', ['bernoulli'] * self.L)))
-        if tc_ok:
+                 all(k in ('bernoulli', 'multinomial') for k in h_kinds))
+        if tc_ok and all(k == 'bernoulli' for k in h_kinds):
             compute = cfg.get('compute') or os.environ.get('BM_DBM_COMPUTE') or os.environ.get('BM_COMPUTE') or 'bf16'
+        elif tc_ok:
+            compute = cfg.get('compute') or os.environ.get('BM_DBM_COMPUTE') or 'fp32'
         self.compute = compute
         c.compute = COMPUTE[compute]
         c.n_particles, c.batch_size = self.M, self.B

@@ -747,4 +747,30 @@ int bm_dbm_ais_rows(bm_dbm* h, int32_t n_runs, int32_t n_betas, int32_t k, uint6
     BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(logZ, "null argument"); DBM(h)->ais_rows(n_runs, n_betas, k, seed, first_run, logZ); BM_API_END
 }
 
+int bm_debug_dbm_multinomial_rows(bm_ctx* hctx, const float* pre, int32_t rows, int32_t cols, double n_samples, int32_t n_draws,
+                                  uint64_t seed, uint32_t site, uint32_t t, uint32_t tick, uint16_t* out_bf, float* out_f32,
+                                  float* ref_means, float* ref_counts) {
+    BM_API_BEGIN
+    Ctx* ctx = reinterpret_cast<Ctx*>(hctx);
+    BM_REQUIRE(ctx && pre && out_bf && out_f32 && ref_means && rows > 0 && cols > 0 && n_draws >= 0, "bad argument");
+    BM_REQUIRE(n_draws == 0 || ref_counts, "bad argument");
+    BM_CUDA(cudaSetDevice(ctx->device));
+    const size_t n = (size_t)rows * cols;
+    DevBuf<float> x, ref, cnt, f32;
+    DevBuf<bf16_t> bf;
+    x.ensure(n); ref.ensure(n); cnt.ensure(n); f32.ensure(n); bf.ensure(n);
+    BM_CUDA(cudaMemcpyAsync(x.p, pre, n * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    BM_CUDA(cudaMemcpyAsync(ref.p, pre, n * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    const RngKey rng = make_rng(seed, site, t, tick, 0);
+    launch_dbm_multinomial_rows(ctx, x.p, cols, rows, cols, (float)n_samples, n_draws, bf.p, cols, f32.p, cols, rng);
+    launch_softmax_rows<float>(ctx, ref.p, cols, rows, cols, (float)n_samples);
+    if (n_draws > 0) launch_multinomial_rows<float>(ctx, ref.p, cols, rows, cols, n_draws, cnt.p, cols, rng);
+    BM_CUDA(cudaMemcpyAsync(out_bf, bf.p, n * sizeof(bf16_t), cudaMemcpyDeviceToHost, ctx->stream));
+    BM_CUDA(cudaMemcpyAsync(out_f32, f32.p, n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    BM_CUDA(cudaMemcpyAsync(ref_means, ref.p, n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    if (n_draws > 0) BM_CUDA(cudaMemcpyAsync(ref_counts, cnt.p, n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    BM_CUDA(cudaStreamSynchronize(ctx->stream));
+    BM_API_END
+}
+
 }  // extern "C"

@@ -12,9 +12,11 @@
 //   softplus(b z) - softplus(a z) = log1p(sigmoid(a z) * expm1((b - a) z)),
 // which is exact to fp32 rounding of a SMALL quantity (no cancellation between two O(1) softplus values).
 //
-// STATUS: the default engine of float32 DBMs (bm_dbm_cfg.compute = BM_COMPUTE_BF16, which the Python mirror passes unless
-// compute='fp32' or BM_DBM_COMPUTE / BM_COMPUTE = fp32 asks for the storage-precision CUDA-core engine).  Models it does not
-// support (DbmTC::supports) run on that engine.
+// STATUS: the default engine of float32 DBMs with Bernoulli hidden layers (bm_dbm_cfg.compute = BM_COMPUTE_BF16, which the
+// Python mirror passes unless compute='fp32' or BM_DBM_COMPUTE / BM_COMPUTE = fp32 asks for the storage-precision CUDA-core
+// engine).  Multinomial hidden layers run here too (dbm_multinomial_rows_kernel after an fp32 pre-activation op); the Python
+// mirror sends such models here only on an explicit compute='bf16' or BM_DBM_COMPUTE=bf16.  Models it does not support
+// (DbmTC::supports) run on the CUDA-core engine.
 #pragma once
 #include <map>
 #include <memory>
@@ -43,6 +45,95 @@ __global__ void mf_chunk_diffs_kernel(const bf16_t* __restrict__ hist, size_t sl
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((threadIdx.x & 31) == 0) atomicMax(flags + j, __float_as_uint(m));
+}
+
+// The conditional of a multinomial layer from its fp32 pre-activations x + b (layers.py:65-70), one row per 256-thread block:
+//   means = scale * softmax(row)                                     softmax_rows_kernel<float> (bm_simt.cu)
+//   n_draws > 0: the counts of n_draws categorical draws of the row   multinomial_rows_kernel<float> on those means
+// and the result leaves as the bf16 GEMM operand `out` (ldo) and, when out_f32 is given, in fp32 as well (ldf): the layer's
+// persistent particles, whose counts stay exact integers above 256 where the bf16 operand rounds them.
+// Bit-identical to the two kernels in sequence: the max and the double sum of the exponentials are reduced in their order (256
+// strided partials, then the same tree), and one thread accumulates the row sum and the CDF sequentially, like theirs.
+// Dynamic shared memory: the row (fp32), and for draws its CDF (fp64, 8-byte aligned) and the counts (int).
+__global__ void __launch_bounds__(256) dbm_multinomial_rows_kernel(const float* __restrict__ pre, int ldp, int cols, float scale,
+                                                                    int n_draws, bf16_t* __restrict__ out, int ldo,
+                                                                    float* __restrict__ out_f32, int ldf, RngKey rng) {
+    extern __shared__ __align__(16) unsigned char mult_smem[];
+    float* x = reinterpret_cast<float*>(mult_smem);
+    double* cdf = reinterpret_cast<double*>(mult_smem + ((size_t)cols * sizeof(float) + 7) / 8 * 8);
+    int* cnt = reinterpret_cast<int*>(cdf + cols);
+    __shared__ double sh[256];
+    const int r = blockIdx.x, tid = threadIdx.x;
+    const float* row = pre + (size_t)r * ldp;
+    double mx = -1e300;
+    for (int c = tid; c < cols; c += 256) { const float v = row[c]; x[c] = v; mx = fmax(mx, (double)v); }
+    sh[tid] = mx;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (tid < o) sh[tid] = fmax(sh[tid], sh[tid + o]);
+        __syncthreads();
+    }
+    const float m = (float)sh[0];
+    __syncthreads();
+    double s = 0.0;
+    for (int c = tid; c < cols; c += 256) { const float e = expf(x[c] - m); x[c] = e; s += (double)e; }
+    sh[tid] = s;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (tid < o) sh[tid] += sh[tid + o];
+        __syncthreads();
+    }
+    const float tot = (float)sh[0];
+    for (int c = tid; c < cols; c += 256) x[c] = scale * x[c] / tot;
+    if (n_draws <= 0) {
+        for (int c = tid; c < cols; c += 256) {
+            out[(size_t)r * ldo + c] = __float2bfloat16_rn(x[c]);
+            if (out_f32) out_f32[(size_t)r * ldf + c] = x[c];
+        }
+        return;
+    }
+    for (int c = tid; c < cols; c += 256) cnt[c] = 0;
+    __syncthreads();
+    if (tid == 0) {
+        double t = 0.0;
+        for (int c = 0; c < cols; ++c) t += (double)x[c];
+        double run = 0.0;
+        for (int c = 0; c < cols; ++c) { run += (double)(float)((double)x[c] / t); cdf[c] = run; }
+    }
+    __syncthreads();
+    const double last = cdf[cols - 1];
+    __syncthreads();
+    for (int c = tid; c < cols; c += 256) cdf[c] = cdf[c] / last;
+    __syncthreads();
+    for (int d = tid; d < n_draws; d += 256) {
+        const U4 w = site_block(rng, (uint32_t)r, (uint32_t)(d >> 2));
+        const uint32_t words[4] = {w.x, w.y, w.z, w.w};
+        const double u = (double)u32_to_unit_float(words[d & 3]);
+        int lo = 0, hi = cols;                                    // first index with cdf > u
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (cdf[mid] > u) hi = mid; else lo = mid + 1;
+        }
+        atomicAdd(&cnt[lo < cols ? lo : cols - 1], 1);
+    }
+    __syncthreads();
+    for (int c = tid; c < cols; c += 256) {
+        const float k = (float)cnt[c];
+        out[(size_t)r * ldo + c] = __float2bfloat16_rn(k);
+        if (out_f32) out_f32[(size_t)r * ldf + c] = k;
+    }
+}
+static inline size_t dbm_multinomial_smem(int cols, bool draws) {
+    return ((size_t)cols * sizeof(float) + 7) / 8 * 8 + (draws ? (size_t)cols * (sizeof(double) + sizeof(int)) : 0);
+}
+void launch_dbm_multinomial_rows(Ctx* ctx, const float* pre, int ldp, int rows, int cols, float scale, int n_draws,
+                                 bf16_t* out, int ldo, float* out_f32, int ldf, RngKey rng) {
+    if (rows <= 0) return;
+    const size_t smem = dbm_multinomial_smem(cols, n_draws > 0);
+    if (smem > 48 * 1024)
+        BM_CUDA(cudaFuncSetAttribute(dbm_multinomial_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    dbm_multinomial_rows_kernel<<<rows, 256, smem, ctx->stream>>>(pre, ldp, cols, scale, n_draws, out, ldo, out_f32, ldf, rng);
+    count_launch(ctx);
 }
 
 // dst[c, r] = bf16(src[r, c]): the transposed bf16 shadow of a weight matrix (src [rows, cols] dense fp32, dst leading dimension ldd)
@@ -189,22 +280,37 @@ struct DbmTC : Dbm<float> {
     DevBuf<bf16_t> Xb, recon_b, v_b, v2_b, v3_b;
     std::vector<DevBuf<bf16_t>> mu_b, h_b, h2_b, h3_b;
     std::vector<DevBuf<float>> Gp;               // split-K slices of the gradient GEMMs
+    // The fp32 copy h[i] of a multinomial layer's particles is never widened from bf16: it holds what set_param /
+    // init_particles put there, then what the row kernel writes on every committed sweep (exact counts, where the bf16
+    // operand rounds above 256).  Only the other layers' copies are widened from bf16 on demand.
     bool particles_f32_stale = false;            // the bf16 particles are newer than the fp32 copies get_param reads
+    DevBuf<float> pre_f32;                       // fp32 pre-activations of a multinomial layer's conditional [max(B, M), H]
+
+    // A multinomial conditional needs whole rows: its op writes fp32 pre-activations (ACT_LINEAR) and one row kernel turns
+    // them into means / counts.  A chain of ops is therefore cut after every such op: the ops between two cuts run as one
+    // program launch, the row kernel between two launches, all in stream order.  Without multinomial layers a chain is one
+    // program, exactly as the ops were listed.
+    struct RowStep { int layer = -1; bf16_t* out = nullptr; float* out_f32 = nullptr; int rows = 0; bool sample = false; uint32_t site = 0, t = 0; };
+    struct TcChain { std::vector<std::unique_ptr<TcProgram>> progs; std::vector<RowStep> after; };
     // mean-field as persistent dataflow programs of up to MF_CHUNK speculated sweeps per launch: slot history + programs
     static constexpr int MF_CHUNK = 5;
     int mf_chunk = 0;                            // MF_CHUNK, clamped by max_mf and by TC_PROGRAM_OPS, at least 1
     std::vector<DevBuf<bf16_t>> hist;            // per layer: (mf_chunk + 2) slots of [B, ldn[i+1]]
     DevBuf<unsigned int> mf_flags;
-    std::map<std::pair<int, int>, std::unique_ptr<TcProgram>> mf_progs;      // keyed by (rows, sweeps in the chunk)
+    std::map<std::pair<int, int>, TcChain> mf_progs;                         // keyed by (rows, sweeps in the chunk)
     // committed particle sweeps as ONE persistent program: keyed by (sweeps, sampled, t0)
-    std::map<std::tuple<int, int, int>, std::unique_ptr<TcProgram>> pcd_progs;
+    std::map<std::tuple<int, int, int>, TcChain> pcd_progs;
 
+    // float32; Bernoulli or Gaussian visibles; Bernoulli and multinomial hidden layers in any order (the DBM's multinomial
+    // particles are refused on a sharded context by init_particles)
     static bool supports(const bm_dbm_cfg& f) {
         if (f.dtype != BM_DTYPE_F32) return false;
         if (!(f.v_kind == BM_UNIT_BERNOULLI || f.v_kind == BM_UNIT_GAUSSIAN)) return false;
-        for (int i = 0; i < f.n_layers; ++i) if (f.h_kinds[i] != BM_UNIT_BERNOULLI) return false;
+        for (int i = 0; i < f.n_layers; ++i)
+            if (f.h_kinds[i] != BM_UNIT_BERNOULLI && f.h_kinds[i] != BM_UNIT_MULTINOMIAL) return false;
         return f.n_layers <= TC_PROGRAM_OPS;     // one mean-field sweep (L ops) fits in one program
     }
+    bool multinomial(int i) const { return h_kinds[i] == BM_UNIT_MULTINOMIAL; }
 
     DbmTC(Ctx* c, const bm_dbm_cfg& f) : Dbm<float>(c, f) {
         ldn.push_back(dbm_round_up(V, 64));
@@ -224,6 +330,9 @@ struct DbmTC : Dbm<float> {
         hist.resize(L);
         for (int i = 0; i < L; ++i) { hist[i].ensure((size_t)(mf_chunk + 2) * B * ldn[i + 1]); hist[i].zero(ctx->stream); }
         mf_flags.ensure(mf_chunk);
+        int hmax = 0;
+        for (int i = 0; i < L; ++i) if (multinomial(i)) hmax = std::max(hmax, Hs[i]);
+        if (hmax) pre_f32.ensure((size_t)std::max(B, M) * hmax);
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
     }
 
@@ -259,7 +368,8 @@ struct DbmTC : Dbm<float> {
     void widen_particles() {
         if (!particles_f32_stale) return;
         launch_bf16_to_f32(ctx, v_b.p, ldn[0], v.p, V, M, V);
-        for (int i = 0; i < L; ++i) launch_bf16_to_f32(ctx, h_b[i].p, ldn[i + 1], h[i].p, Hs[i], M, Hs[i]);
+        for (int i = 0; i < L; ++i)
+            if (!multinomial(i)) launch_bf16_to_f32(ctx, h_b[i].p, ldn[i + 1], h[i].p, Hs[i], M, Hs[i]);
         particles_f32_stale = false;
     }
     void widen_mu(int rows) { for (int i = 0; i < L; ++i) launch_bf16_to_f32(ctx, mu_b[i].p, ldn[i + 1], mu[i].p, Hs[i], rows, Hs[i]); }
@@ -282,10 +392,17 @@ struct DbmTC : Dbm<float> {
     }
 
     // ---- one fused conditional on the tensor cores -----------------------------------------------------------
-    // act(acc_scale * (below W_i [+ above W_{i+1}^T]) + bias_scale * b_i): means XOR sampled states (bf16)
+    // act(acc_scale * (below W_i [+ above W_{i+1}^T]) + bias_scale * b_i): means XOR sampled states (bf16).  A multinomial
+    // layer's op leaves x + b in pre_f32 and the row kernel writes `out` (and, given out_f32, the fp32 particles)
     void hidden_tc(int i, const bf16_t* below, const bf16_t* above, bf16_t* out, bool sample, int rows,
-                   float acc_scale, float bias_scale, RngKey rng) {
+                   float acc_scale, float bias_scale, RngKey rng, float* out_f32 = nullptr) {
         launch_tc_gemm(ctx, hidden_gemm(i, below, above, out, sample, rows, acc_scale, bias_scale, rng));
+        if (multinomial(i)) multinomial_rows(i, rows, out, out_f32, sample, rng);
+    }
+    void multinomial_rows(int i, int rows, bf16_t* out, float* out_f32, bool sample, RngKey rng) {
+        const int n = (int)h_n_samples[i];
+        launch_dbm_multinomial_rows(ctx, pre_f32.p, Hs[i], rows, Hs[i], (float)h_n_samples[i], sample ? n : 0, out, ldn[i + 1],
+                                    out_f32, Hs[i], rng);
     }
     TcGemm hidden_gemm(int i, const bf16_t* below, const bf16_t* above, bf16_t* out, bool sample, int rows,
                        float acc_scale, float bias_scale, RngKey rng) {
@@ -296,6 +413,7 @@ struct DbmTC : Dbm<float> {
         g.B[0] = mat(Wb[i].p, in, H, ldn[i + 1]); g.b_t[0] = true;           // x W_i: W_i stored [K, N]
         if (above) above_pair(g, i, above, rows);
         g.acc_scale = acc_scale; g.bias_scale = bias_scale; g.bias = hb[i].p;
+        if (multinomial(i)) { g.act = ACT_LINEAR; g.out_f32 = pre_f32.p; g.ld_f32 = H; return g; }     // layers.py:65-66
         g.act = ACT_SIGMOID; g.rng = rng;
         if (sample) { g.sample = SMP_BERNOULLI; g.out_state_bf = out; g.ld_state_bf = ldn[i + 1]; }
         else { g.out_mean_bf = out; g.ld_mean_bf = ldn[i + 1]; }
@@ -333,11 +451,12 @@ struct DbmTC : Dbm<float> {
 
     // dbm.py:385-427 on bf16 operands.  Hn[i] receive the new hidden values (states when sampled, else means)
     void gibbs_tc(const bf16_t* vin, const std::vector<const bf16_t*>& Hin, const std::vector<bf16_t*>& Hn, bf16_t* v_new,
-                  bool update_v, bool sample, int rows, uint64_t seed, uint32_t tstep, uint32_t tick) {
+                  bool update_v, bool sample, int rows, uint64_t seed, uint32_t tstep, uint32_t tick, bool commit) {
         for (int i = 0; i < L; ++i) {
             const bf16_t* below = i == 0 ? vin : Hn[i - 1];
             const bf16_t* above = (i + 1 < L) ? Hin[i + 1] : nullptr;
-            hidden_tc(i, below, above, Hn[i], sample && sample_h[i], rows, 1.f, 1.f, make_rng(seed, SITE_DBM_H + i, tstep, tick, particle_row0()));
+            hidden_tc(i, below, above, Hn[i], sample && sample_h[i], rows, 1.f, 1.f, make_rng(seed, SITE_DBM_H + i, tstep, tick, particle_row0()),
+                      commit ? h[i].p : nullptr);
         }
         if (update_v) visible_tc(Hn[0], v_new, sample && sample_vis, rows, make_rng(seed, SITE_DBM_V, tstep, tick, particle_row0()));
     }
@@ -346,6 +465,38 @@ struct DbmTC : Dbm<float> {
         const float* X = upload(Xh, rows);
         launch_f32_to_bf16(ctx, X, V, Xb.p, ldn[0], rows, V);
         return X;
+    }
+
+    // `ops` with dependencies as indices into it; row[k].layer >= 0: a row kernel follows op k.  A dependency on an op of an
+    // earlier launch is dropped: the kernel boundary orders it.
+    static void cut_chain(TcChain& chain, const std::vector<TcGemm>& ops, const std::vector<RowStep>& row) {
+        size_t lo = 0;
+        for (size_t k = 0; k < ops.size(); ++k) {
+            if (row[k].layer < 0 && k + 1 < ops.size()) continue;
+            std::unique_ptr<TcProgram> p(new TcProgram());
+            for (size_t j = lo; j <= k; ++j) {
+                TcGemm g = ops[j];
+                int n = 0;
+                for (int d = 0; d < g.n_deps; ++d)
+                    if (g.dep[d] >= (int)lo) { g.dep[n] = g.dep[d] - (int)lo; g.dep_all[n] = g.dep_all[d]; ++n; }
+                for (int d = n; d < g.n_deps; ++d) { g.dep[d] = -1; g.dep_all[d] = false; }
+                g.n_deps = n;
+                p->ops.push_back(g);
+            }
+            chain.progs.push_back(std::move(p));
+            chain.after.push_back(row[k]);
+            lo = k + 1;
+        }
+    }
+    // the programs get `rng` (seed / tick / row0 shared by their ops); a sampling row kernel draws from (seed, site, t, tick)
+    void run_chain(TcChain& chain, RngKey rng, uint64_t seed, uint32_t tick) {
+        for (size_t k = 0; k < chain.progs.size(); ++k) {
+            launch_tc_program(ctx, *chain.progs[k], rng, 0);
+            const RowStep& st = chain.after[k];
+            if (st.layer >= 0)
+                multinomial_rows(st.layer, st.rows, st.out, st.out_f32, st.sample,
+                                 st.sample ? make_rng(seed, st.site, st.t, tick, particle_row0()) : RngKey{});
+        }
     }
 
     // ---- E-step (dbm.py:429-478) ------------------------------------------------------------------------------
@@ -367,10 +518,10 @@ struct DbmTC : Dbm<float> {
         bool done = false;
         while (!done && a < max_mf) {
             const int c = std::min(mf_chunk, max_mf - a);
-            std::unique_ptr<TcProgram>& pslot = mf_progs[std::make_pair(rows, c)];
-            if (!pslot) {
-                pslot.reset(new TcProgram());
-                std::vector<TcGemm>& ops = pslot->ops;
+            TcChain& chain = mf_progs[std::make_pair(rows, c)];
+            if (chain.progs.empty()) {
+                std::vector<TcGemm> ops;
+                std::vector<RowStep> row;
                 for (int s = 1; s <= c; ++s)                                 // sweep s: slot s -> slot s + 1
                     for (int i = 0; i < L; ++i) {
                         const bf16_t* below = i == 0 ? Xb.p : slot(i - 1, s + 1);
@@ -381,9 +532,13 @@ struct DbmTC : Dbm<float> {
                         if (above && s > 1) { g.dep[g.n_deps] = self - L + 1; g.dep_all[g.n_deps] = false; ++g.n_deps; } // layer i+1, previous sweep
                         g.lane = LANE_CHAIN;
                         ops.push_back(g);
+                        RowStep st;
+                        if (multinomial(i)) { st.layer = i; st.out = slot(i, s + 1); st.rows = rows; }
+                        row.push_back(st);
                     }
+                cut_chain(chain, ops, row);
             }
-            launch_tc_program(ctx, *pslot, RngKey{}, 0);
+            run_chain(chain, RngKey{}, 0, 0);
             BM_CUDA(cudaMemsetAsync(mf_flags.p, 0, (size_t)c * sizeof(unsigned int), ctx->stream));
             for (int i = 0; i < L; ++i) {
                 mf_chunk_diffs_kernel<<<dim3((unsigned)(ctx->sm_count / 2), c), 256, 0, ctx->stream>>>(hist[i].p, (size_t)B * ldn[i + 1], ldn[i + 1], rows, Hs[i], mf_flags.p);
@@ -420,13 +575,13 @@ struct DbmTC : Dbm<float> {
     // PCD-k on an RBM is the reference's DBM with one layer).  Ping-pong buffers: a buffer is overwritten two sweeps
     // after it was written, and every reader of the old value precedes the writer in the dependency chain.
     void particles_program(int n_steps, bool sample, uint64_t seed, uint32_t tick, int t0) {
-        std::unique_ptr<TcProgram>& pslot = pcd_progs[std::make_tuple(n_steps, sample ? 1 : 0, t0)];
+        TcChain& chain = pcd_progs[std::make_tuple(n_steps, sample ? 1 : 0, t0)];
         std::vector<bf16_t*> cur(L), nxt(L);
         for (int i = 0; i < L; ++i) { cur[i] = h_b[i].p; nxt[i] = h2_b[i].p; }
         bf16_t* vc = v_b.p; bf16_t* vn = v2_b.p;
-        const bool build = !pslot;
-        if (build) pslot.reset(new TcProgram());
-        std::vector<TcGemm>& ops = pslot->ops;
+        const bool build = chain.progs.empty();
+        std::vector<TcGemm> ops;
+        std::vector<RowStep> row;
         int last_vis = -1;
         std::vector<int> last_h(L, -1), this_h(L, -1);
         for (int s = 0; s < n_steps; ++s) {
@@ -442,17 +597,25 @@ struct DbmTC : Dbm<float> {
                     g.lane = LANE_CHAIN;
                     this_h[i] = (int)ops.size();
                     ops.push_back(g);
+                    RowStep st;
+                    if (multinomial(i)) {      // committed sweeps: the row kernel also writes the fp32 particles
+                        st.layer = i; st.out = nxt[i]; st.out_f32 = h[i].p; st.rows = M; st.sample = sample && sample_h[i];
+                        st.site = SITE_DBM_H + i; st.t = tstep;
+                    }
+                    row.push_back(st);
                 }
                 TcGemm gv = visible_gemm(nxt[0], vn, sample && sample_vis, M, make_rng(0, SITE_DBM_V, tstep, 0, 0));
                 gv.dep[0] = this_h[0]; gv.dep_all[0] = false; gv.n_deps = 1;
                 gv.lane = LANE_CHAIN;
                 last_vis = (int)ops.size();
                 ops.push_back(gv);
+                row.push_back(RowStep());
                 last_h = this_h;
             }
             std::swap(cur, nxt); std::swap(vc, vn);
         }
-        launch_tc_program(ctx, *pslot, make_rng(seed, 0, 0, tick, particle_row0()), 0);
+        if (build) cut_chain(chain, ops, row);
+        run_chain(chain, make_rng(seed, 0, 0, tick, particle_row0()), seed, tick);
         for (int i = 0; i < L; ++i)
             if (cur[i] != h_b[i].p)
                 BM_CUDA(cudaMemcpyAsync(h_b[i].p, cur[i], (size_t)M * ldn[i + 1] * sizeof(bf16_t), cudaMemcpyDeviceToDevice, ctx->stream));
@@ -477,7 +640,7 @@ struct DbmTC : Dbm<float> {
         }
         for (int s = 0; s < n_steps; ++s) {
             std::vector<const bf16_t*> Hin(cur.begin(), cur.end());
-            gibbs_tc(vc, Hin, nxt, vn, true, sample, M, seed, (uint32_t)(t0 + s + 1), tick);
+            gibbs_tc(vc, Hin, nxt, vn, true, sample, M, seed, (uint32_t)(t0 + s + 1), tick, commit);
             if (!commit && s == 0) { cur = nxt; nxt = spare; vc = vn; vn = vspare; }
             else { std::swap(cur, nxt); std::swap(vc, vn); }
         }
@@ -596,6 +759,7 @@ struct DbmTC : Dbm<float> {
     }
     void log_proba(const void* Xh, int rows, double* out) override {
         BM_REQUIRE(L == 2, "log_proba is defined for 2 hidden layers");
+        BM_REQUIRE(!multinomial(0) && !multinomial(1), "log_proba is defined for binary hidden layers (dbm.py:946-948)");
         const float* X = upload_tc(Xh, rows);
         mean_field_tc(rows);
         linear_tc(Xb.p, ldn[0], rows, V, Wb[0].p, V, Hs[0], ldn[1], true, Hs[0], nullptr, t[0].p);              // t1 = X W_0

@@ -160,7 +160,8 @@ typedef struct bm_dbm_cfg {
     int32_t v_kind;                  /* BM_UNIT_*                                          */
     const int32_t* h_kinds;
     const double*  h_n_samples;      /* MultinomialLayer.n_samples per layer (nullable)    */
-    int32_t dtype, compute;          /* BM_COMPUTE_BF16: tensor-core engine (F32 models, Bernoulli hidden layers) */
+    int32_t dtype, compute;          /* BM_COMPUTE_BF16: tensor-core engine (F32 models, Bernoulli or Gaussian visibles,
+                                        Bernoulli and multinomial hidden layers); other models run on the FP32 engine */
     int32_t n_particles, batch_size, max_mf_updates;
     int32_t sample_v;
     const int32_t* sample_h;
@@ -257,6 +258,15 @@ typedef struct bm_tc_op_plan {
     int32_t follows_granules;              /* 1: waits for its producer's 64-column granules one by one */
 } bm_tc_op_plan;
 int  bm_rbm_debug_tc_plan(bm_rbm* rbm, bm_tc_op_plan* out, int32_t cap, int32_t* n_ops);
+
+/* ---- test hook: the multinomial conditional of the tensor-core DBM engine ---------------------
+ * From host fp32 pre-activations pre [rows, cols] (x + b of the layer), the engine's fused row kernel writes
+ * n_samples * softmax(row) -- or, n_draws > 0, the counts of n_draws categorical draws from Philox (seed, site | t << 8,
+ * tick, row r) -- as bf16 bit patterns to out_bf and in fp32 to out_f32 (both [rows, cols]); from the same input the
+ * CUDA-core engine's two kernels write their fp32 means to ref_means and their counts to ref_counts (n_draws > 0). */
+int  bm_debug_dbm_multinomial_rows(bm_ctx* ctx, const float* pre, int32_t rows, int32_t cols, double n_samples, int32_t n_draws,
+                                   uint64_t seed, uint32_t site, uint32_t t, uint32_t tick, uint16_t* out_bf, float* out_f32,
+                                   float* ref_means, float* ref_counts);
 
 #ifdef __cplusplus
 }
