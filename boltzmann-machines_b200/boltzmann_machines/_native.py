@@ -31,6 +31,8 @@ EXPORTS = (
     'bm_dbm_create', 'bm_dbm_destroy', 'bm_dbm_set_param', 'bm_dbm_get_param', 'bm_dbm_init_particles',
     'bm_dbm_train_step', 'bm_dbm_val_metrics', 'bm_dbm_transform', 'bm_dbm_reconstruct', 'bm_dbm_log_proba',
     'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows', 'bm_debug_dbm_multinomial_rows',
+    'bm_crbm_create', 'bm_crbm_destroy', 'bm_crbm_set_param', 'bm_crbm_get_param', 'bm_crbm_init_weights',
+    'bm_crbm_train_step', 'bm_crbm_predict_proba', 'bm_crbm_transform',
 )
 
 
@@ -64,6 +66,17 @@ class DbmCfg(C.Structure):
         ('sparsity_target', C.POINTER(C.c_double)),
         ('sparsity_cost', C.POINTER(C.c_double)),
         ('sigma', C.POINTER(C.c_double)),
+    ]
+
+
+class CrbmCfg(C.Structure):
+    _fields_ = [
+        ('n_visible', C.c_int32), ('n_hidden', C.c_int32), ('n_classes', C.c_int32),
+        ('dtype', C.c_int32), ('compute', C.c_int32),
+        ('sample_v', C.c_int32), ('sample_h', C.c_int32),
+        ('max_batch', C.c_int32),
+        ('alpha', C.c_double), ('l2', C.c_double), ('dropout_keep', C.c_double), ('sparsity_cost', C.c_double),
+        ('dbm_first', C.c_int32), ('dbm_last', C.c_int32),
     ]
 
 
@@ -144,6 +157,11 @@ def load_library(path=None):
         'bm_dbm_ais': [vp, i32, i32, i32, u64, vp],
         'bm_dbm_ais_rows': [vp, i32, i32, i32, u64, u32, vp],
         'bm_debug_dbm_multinomial_rows': [vp, vp, i32, i32, dbl, i32, u64, u32, u32, u32, vp, vp, vp, vp],
+        'bm_crbm_create': [vp, C.POINTER(CrbmCfg), C.POINTER(vp)],
+        'bm_crbm_set_param': [vp, C.c_char_p, vp, sz], 'bm_crbm_get_param': [vp, C.c_char_p, vp, sz],
+        'bm_crbm_init_weights': [vp, dbl, u64, u64],
+        'bm_crbm_train_step': [vp, vp, vp, i32, dbl, dbl, i32, u64, u32, i32, C.POINTER(dbl)],
+        'bm_crbm_predict_proba': [vp, vp, i32, vp], 'bm_crbm_transform': [vp, vp, i32, vp],
     }
     for name, argtypes in protos.items():
         fn = getattr(lib, name)
@@ -155,6 +173,8 @@ def load_library(path=None):
     lib.bm_rbm_destroy.restype = None
     lib.bm_dbm_destroy.argtypes = [vp]
     lib.bm_dbm_destroy.restype = None
+    lib.bm_crbm_destroy.argtypes = [vp]
+    lib.bm_crbm_destroy.restype = None
     if path is None:
         _lib = lib
     return lib
@@ -770,10 +790,104 @@ class CudaDBM(object):
             pass
 
 
+class CudaCRBM(object):
+    """Engine object for ``ClassificationRBM``: a ``bm_crbm`` handle (csrc/bm_crbm_tc.cuh, tensor cores only).
+
+    cfg: n_visible, n_hidden, n_classes, alpha, l2, sample_v, sample_h, max_batch, and dtype / compute / dropout /
+    sparsity_cost / dbm_first / dbm_last, which the engine refuses unless they are float32 / bf16 / None / 0 / False /
+    False."""
+
+    def __init__(self, cfg, ctx=None):
+        self._lib = load_library()
+        self.ctx = ctx or Context.default()
+        self.cfg = dict(cfg)
+        self.V, self.H, self.C = int(cfg['n_visible']), int(cfg['n_hidden']), int(cfg['n_classes'])
+        self.dt = np.dtype(cfg.get('dtype', 'float32'))
+        c = CrbmCfg()
+        c.n_visible, c.n_hidden, c.n_classes = self.V, self.H, self.C
+        c.dtype = DTYPES[self.dt.name]
+        c.compute = COMPUTE[cfg.get('compute') or os.environ.get('BM_COMPUTE') or 'bf16']
+        c.sample_v, c.sample_h = int(cfg.get('sample_v', False)), int(cfg.get('sample_h', True))
+        c.max_batch = int(cfg['max_batch'])
+        c.alpha, c.l2 = float(cfg.get('alpha', 0.01)), float(cfg.get('l2', 0.))
+        keep = cfg.get('dropout', None)
+        c.dropout_keep = -1.0 if keep is None else float(keep)
+        c.sparsity_cost = float(cfg.get('sparsity_cost', 0.))
+        c.dbm_first, c.dbm_last = int(bool(cfg.get('dbm_first', False))), int(bool(cfg.get('dbm_last', False)))
+        h = C.c_void_p()
+        rc = self._lib.bm_crbm_create(self.ctx.handle, C.byref(c), C.byref(h))
+        if rc == -5:                                  # BM_EUNSUPPORTED: the message names the option
+            raise NotImplementedError(self._lib.bm_last_error().decode('utf-8', 'replace'))
+        check(rc)
+        self.handle = h
+        V, H, Cn = self.V, self.H, self.C
+        self._shapes = {'W': (V, H), 'U': (Cn, H), 'vb': (V,), 'hb': (H,), 'yb': (Cn,),
+                        'dW': (V, H), 'dU': (Cn, H), 'dvb': (V,), 'dhb': (H,), 'dyb': (Cn,)}
+        self._out2 = (C.c_double * 2)()
+
+    def set_params(self, d):
+        for k, v in d.items():
+            a = np.ascontiguousarray(v, dtype=np.float32).reshape(self._shapes[k])
+            check(self._lib.bm_crbm_set_param(self.handle, k.encode(), a.ctypes.data, a.nbytes))
+
+    def get_params(self, names=None):
+        out = {}
+        for k in (names or list(self._shapes)):
+            a = np.empty(self._shapes[k], dtype=np.float32)
+            check(self._lib.bm_crbm_get_param(self.handle, k.encode(), a.ctypes.data, a.nbytes))
+            out[k] = a
+        return out
+
+    def init_normal_weights(self, stddev, op_seed_w, op_seed_u):
+        check(self._lib.bm_crbm_init_weights(self.handle, float(stddev), int(op_seed_w) & (2 ** 64 - 1),
+                                             int(op_seed_u) & (2 ** 64 - 1)))
+
+    def _batch(self, X):
+        X = np.ascontiguousarray(X, dtype=np.float32)
+        if X.ndim != 2 or X.shape[1] != self.V:
+            raise ValueError('batch has shape {0}, expected (rows, {1})'.format(X.shape, self.V))
+        return X
+
+    def train_step(self, X, y, lr, momentum, k, seed, tick, metrics=False):
+        """One hybrid step; with ``metrics`` returns {'nll', 'accuracy'} of the batch under the pre-update weights."""
+        X = self._batch(X)
+        y = np.ascontiguousarray(y, dtype=np.int32).reshape(-1)
+        if y.shape[0] != X.shape[0]:
+            raise ValueError('{0} labels for {1} rows'.format(y.shape[0], X.shape[0]))
+        check(self._lib.bm_crbm_train_step(self.handle, X.ctypes.data, y.ctypes.data, X.shape[0], float(lr), float(momentum),
+                                           int(k), int(seed) & (2 ** 64 - 1), int(tick), 1 if metrics else 0, self._out2))
+        return {'nll': float(self._out2[0]), 'accuracy': float(self._out2[1])} if metrics else None
+
+    def predict_proba(self, X):
+        X = self._batch(X)
+        out = np.empty((X.shape[0], self.C), dtype=np.float32)
+        check(self._lib.bm_crbm_predict_proba(self.handle, X.ctypes.data, X.shape[0], out.ctypes.data))
+        return out
+
+    def transform(self, X):
+        X = self._batch(X)
+        out = np.empty((X.shape[0], self.H), dtype=np.float32)
+        check(self._lib.bm_crbm_transform(self.handle, X.ctypes.data, X.shape[0], out.ctypes.data))
+        return out
+
+    def close(self):
+        if getattr(self, 'handle', None):
+            self._lib.bm_crbm_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 def default_factory(kind):
     load_library()
     if kind == 'dbm':
         return CudaDBM
     if kind == 'rbm':
         return CudaRBM
+    if kind == 'crbm':
+        return CudaCRBM
     raise RuntimeError("no native engine for '{0}'".format(kind))

@@ -1,2 +1,3 @@
 from .base_rbm import *
 from .rbm import *
+from .class_rbm import *

@@ -678,6 +678,7 @@ struct Dbm : DbmBase {
 }  // namespace bm
 
 #include "bm_dbm_tc.cuh"     // DbmTC: the same engine with every GEMM on the tensor cores (opt-in)
+#include "bm_crbm_tc.cuh"    // ClassRbmTC: the classification RBM, a DbmTC of shape x - h - label (bm_crbm_*)
 
 using namespace bm;
 

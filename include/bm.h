@@ -268,6 +268,39 @@ int  bm_debug_dbm_multinomial_rows(bm_ctx* ctx, const float* pre, int32_t rows, 
                                    uint64_t seed, uint32_t site, uint32_t t, uint32_t tick, uint16_t* out_bf, float* out_f32,
                                    float* ref_means, float* ref_counts);
 
+/* ---- Classification RBM (Larochelle & Bengio, ICML 2008; no counterpart in the reference) -------------
+ * Visible x [n_visible] and a one-of-n_classes label beside it, both connected to h [n_hidden]:
+ * E = -x'W h - e_y'U h - vb'x - hb'h - yb'e_y.  p(y|x) is exact; training takes the hybrid gradient
+ * grad = d/dtheta mean log p(t|x) + alpha * (CD-k on the joint p(x, y)) - l2 * (W, U), then the momentum update
+ * d <- lr (momentum d + grad), theta += d.  Runs on the tensor cores only: float32 models, BM_COMPUTE_BF16.
+ * BM_EUNSUPPORTED (with the option named) for float64, BM_COMPUTE_FP32, dropout, a sparsity cost, dbm_first /
+ * dbm_last and a context with a communicator; BM_EINVAL unless 2 <= n_classes <= 64. */
+typedef struct bm_crbm bm_crbm;
+typedef struct bm_crbm_cfg {
+    int32_t n_visible, n_hidden, n_classes;
+    int32_t dtype, compute;          /* BM_DTYPE_F32 / BM_COMPUTE_BF16: anything else is refused */
+    int32_t sample_v, sample_h;      /* sample_v_states (x and label draws in the chain) / sample_h_states */
+    int32_t max_batch;               /* rows of the largest batch (workspaces are sized once) */
+    double  alpha;                   /* weight of the generative gradient; 0: purely discriminative, no chain */
+    double  l2;
+    double  dropout_keep;            /* < 0 (none); anything else is refused */
+    double  sparsity_cost;           /* 0; anything else is refused */
+    int32_t dbm_first, dbm_last;     /* 0; anything else is refused */
+} bm_crbm_cfg;
+int  bm_crbm_create(bm_ctx* ctx, const bm_crbm_cfg* cfg, bm_crbm** out);
+void bm_crbm_destroy(bm_crbm* crbm);
+/* variables "W" [V,H], "U" [C,H], "vb" [V], "hb" [H], "yb" [C] and their momenta "dW", "dU", "dvb", "dhb", "dyb" (float32) */
+int  bm_crbm_set_param(bm_crbm* crbm, const char* name, const void* host, size_t bytes);
+int  bm_crbm_get_param(bm_crbm* crbm, const char* name, void* host, size_t bytes);
+/* W <- N(0, stddev) from tf.random_normal's stream of op_seed_w, U [C,H] likewise from op_seed_u */
+int  bm_crbm_init_weights(bm_crbm* crbm, double stddev, uint64_t op_seed_w, uint64_t op_seed_u);
+/* one hybrid step on X [rows, n_visible] (float32) with labels [rows] in [0, n_classes) (BM_EINVAL before any launch
+ * otherwise); 1 <= rows <= max_batch.  want_metrics != 0: out2 = {mean -log p(t|x), accuracy} under the pre-update weights */
+int  bm_crbm_train_step(bm_crbm* crbm, const void* X, const int32_t* labels, int32_t rows, double lr, double momentum,
+                        int32_t n_gibbs_steps, uint64_t seed, uint32_t tick, int32_t want_metrics, double* out2);
+int  bm_crbm_predict_proba(bm_crbm* crbm, const void* X, int32_t rows, float* out);    /* p(y|x): out [rows, n_classes] */
+int  bm_crbm_transform(bm_crbm* crbm, const void* X, int32_t rows, float* out);        /* E[h|x]: out [rows, n_hidden]  */
+
 #ifdef __cplusplus
 }
 #endif
