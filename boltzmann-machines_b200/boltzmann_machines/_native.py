@@ -77,6 +77,7 @@ class CrbmCfg(C.Structure):
         ('max_batch', C.c_int32),
         ('alpha', C.c_double), ('l2', C.c_double), ('dropout_keep', C.c_double), ('sparsity_cost', C.c_double),
         ('dbm_first', C.c_int32), ('dbm_last', C.c_int32),
+        ('beta', C.c_double),
     ]
 
 
@@ -793,7 +794,8 @@ class CudaDBM(object):
 class CudaCRBM(object):
     """Engine object for ``ClassificationRBM``: a ``bm_crbm`` handle (csrc/bm_crbm_tc.cuh, tensor cores only).
 
-    cfg: n_visible, n_hidden, n_classes, alpha, l2, sample_v, sample_h, max_batch, and dtype / compute / dropout /
+    cfg: n_visible, n_hidden, n_classes, alpha, beta (labels of -1 mark unlabelled rows when beta > 0), l2, sample_v,
+    sample_h, max_batch, and dtype / compute / dropout /
     sparsity_cost / dbm_first / dbm_last, which the engine refuses unless they are float32 / bf16 / None / 0 / False /
     False."""
 
@@ -814,6 +816,7 @@ class CudaCRBM(object):
         c.dropout_keep = -1.0 if keep is None else float(keep)
         c.sparsity_cost = float(cfg.get('sparsity_cost', 0.))
         c.dbm_first, c.dbm_last = int(bool(cfg.get('dbm_first', False))), int(bool(cfg.get('dbm_last', False)))
+        c.beta = float(cfg.get('beta', 0.))
         h = C.c_void_p()
         rc = self._lib.bm_crbm_create(self.ctx.handle, C.byref(c), C.byref(h))
         if rc == -5:                                  # BM_EUNSUPPORTED: the message names the option

@@ -6,6 +6,10 @@ of the batch mean of log p(t|x) plus ``alpha`` times CD-k on the joint p(x, y) (
 runs no Gibbs chain; the default 0.01 is the value the paper reports for MNIST), minus ``l2`` times W and U, applied with
 the momentum update of BaseRBM.  The whole step runs in one native call (``bm_crbm_train_step``, csrc/bm_crbm_tc.cuh) on
 the tensor cores.
+
+Semi-supervised training (Larochelle, Mandel, Pascanu & Bengio, JMLR 13, 2012): with ``beta > 0`` a label of -1 marks an
+unlabelled row, which adds ``beta`` times CD-k of log p(x) -- an exact positive phase and a chain started from a label drawn
+from p(y|x) -- so unlabelled data shapes the same joint model the labels train.
 """
 import numpy as np
 
@@ -31,6 +35,8 @@ class ClassificationRBM(EnergyBasedModel):
     n_visible, n_hidden : positive int
     n_classes : int in [2, 64]
     alpha : weight of the generative (CD-k on p(x, y)) gradient; 0 trains purely discriminatively
+    beta : weight of the unlabelled rows' gradient (CD-k on p(x)); with beta > 0, ``fit`` accepts -1 in ``y`` for a row
+        without a label.  0 (the default) accepts labelled rows only
     W_init : float (std of the N(0, .) init of W and U) or (n_visible, n_hidden) array for W
     U_init : None (drawn like W from its own op seed) or (n_classes, n_hidden) array
     vb_init, hb_init, yb_init : float or array
@@ -54,7 +60,7 @@ class ClassificationRBM(EnergyBasedModel):
                  sample_v_states=False, sample_h_states=True,
                  dropout=None, sparsity_cost=0., dbm_first=False, dbm_last=False, compute=None,
                  metrics_config=None, verbose=True, save_after_each_epoch=True,
-                 model_path='class_rbm_model/', *args, **kwargs):
+                 model_path='class_rbm_model/', beta=0., *args, **kwargs):
         super(ClassificationRBM, self).__init__(model_path=model_path, *args, **kwargs)
         for name, value, default in (('dropout', dropout, None), ('sparsity_cost', sparsity_cost, 0.),
                                      ('dbm_first', dbm_first, False), ('dbm_last', dbm_last, False)):
@@ -68,6 +74,9 @@ class ClassificationRBM(EnergyBasedModel):
             raise ValueError('n_classes must be in [2, 64], got {0}'.format(n_classes))
         self.n_visible, self.n_hidden, self.n_classes = n_visible, n_hidden, n_classes
         self.alpha = alpha
+        if not float(beta) >= 0.:
+            raise ValueError('beta must be non-negative, got {0!r}'.format(beta))
+        self.beta = beta
         self.dropout, self.sparsity_cost, self.dbm_first, self.dbm_last, self.compute = \
             dropout, sparsity_cost, dbm_first, dbm_last, compute
 
@@ -109,7 +118,7 @@ class ClassificationRBM(EnergyBasedModel):
     # ---- engine wiring ---------------------------------------------------------------
     def _engine_cfg(self):
         return dict(n_visible=int(self.n_visible), n_hidden=int(self.n_hidden), n_classes=int(self.n_classes),
-                    alpha=float(self.alpha), l2=float(self.l2), dtype=self.dtype, compute=self.compute,
+                    alpha=float(self.alpha), beta=float(self.beta), l2=float(self.l2), dtype=self.dtype, compute=self.compute,
                     sample_v=bool(self.sample_v_states), sample_h=bool(self.sample_h_states),
                     max_batch=int(self.batch_size), dropout=self.dropout, sparsity_cost=float(self.sparsity_cost),
                     dbm_first=bool(self.dbm_first), dbm_last=bool(self.dbm_last))
@@ -142,12 +151,18 @@ class ClassificationRBM(EnergyBasedModel):
     def _scheduled(self, values):
         return values[min(self.epoch_, len(values) - 1)]
 
-    def _labels(self, y, n):
+    def _labels(self, y, n, unlabelled=False):
+        """y as int32; -1 (a row without a label) is accepted where ``unlabelled`` allows it and beta > 0"""
         y = np.asarray(y).reshape(-1)
         if y.shape[0] != n:
             raise ValueError('{0} labels for {1} rows'.format(y.shape[0], n))
-        if y.size and (y.min() < 0 or y.max() >= self.n_classes or not np.all(y == np.round(y))):
+        if y.size and not np.all(y == np.round(y)):
             raise ValueError('labels must be integers in [0, {0})'.format(self.n_classes))
+        if y.size and unlabelled and y.min() == -1 and not float(self.beta) > 0:
+            raise ValueError('labels of -1 (unlabelled rows) need beta > 0; beta is {0!r}'.format(self.beta))
+        low = -1 if unlabelled and float(self.beta) > 0 else 0
+        if y.size and (y.min() < low or y.max() >= self.n_classes):
+            raise ValueError('labels must be integers in [{0}, {1})'.format(low, self.n_classes))
         return np.ascontiguousarray(y, dtype=np.int32)
 
     def _train_epoch(self, X, y):
@@ -157,7 +172,8 @@ class ClassificationRBM(EnergyBasedModel):
         got = []
         for lo, hi in _maybe_bar(batch_bounds(len(X), self.batch_size), self.verbose, leave=False, ncols=64, desc='epoch'):
             self.iter_ += 1
-            reporting = bool(every and self.iter_ % every == 0)
+            # metrics come from the batch's labelled rows: a reporting batch without one logs nothing
+            reporting = bool(every and self.iter_ % every == 0) and bool(np.any(y[lo:hi] >= 0))
             m = self._engine.train_step(X[lo:hi], y[lo:hi], lr, mom, k, self._call_seed, self._next_tick(), metrics=reporting)
             if reporting:
                 got.append(m)
@@ -176,7 +192,7 @@ class ClassificationRBM(EnergyBasedModel):
         if y is None:
             raise ValueError('ClassificationRBM.fit needs the labels y')
         X = np.ascontiguousarray(X, dtype=np.float32)
-        y = self._labels(y, len(X))
+        y = self._labels(y, len(X), unlabelled=True)
         if X_val is not None:
             X_val = np.ascontiguousarray(X_val, dtype=np.float32)
             y_val = self._labels(y_val, len(X_val))
@@ -197,7 +213,11 @@ class ClassificationRBM(EnergyBasedModel):
                 self._save_model(global_step=self.epoch_)
 
     def fit(self, X, y=None, X_val=None, y_val=None):
-        """Train on X [n, n_visible] with labels y [n] in [0, n_classes); validation data optional."""
+        """Train on X [n, n_visible] with labels y [n] in [0, n_classes); validation data optional.
+
+        With ``beta > 0``, y may hold -1 for rows without a label (``y_val`` must be fully labelled).  Batches are taken in
+        row order, as for labelled data, so the order of X decides how labelled and unlabelled rows share a batch: shuffle
+        or interleave them beforehand to mix them."""
         return super(ClassificationRBM, self).fit(X, X_val=X_val, y=y, y_val=y_val)
 
     # ---- inference -------------------------------------------------------------------------

@@ -20,8 +20,13 @@
 // with s[b,y,j] = sigmoid(o[b,y,j]), S_t[b,j] = s[b,t_b,j] (the positive hidden means of the joint) and
 // S^[b,j] = sum_y p[b,y] s[b,y,j].
 //
-// Draws (Philox, make_rng(seed, site, t, tick, 0)): h0 states SITE_H0 (t = 0); sweep s = 1..k draws x at SITE_V, the label at
-// SITE_CRBM_Y and h at SITE_H, all with t = s (DESIGN.md §3).
+// Semi-supervised rows (Larochelle, Mandel, Pascanu & Bengio, JMLR 2012): with beta > 0 a row labelled -1 adds
+// beta * CD-k of log p(x) instead.  Its positive phase is exact (x S^, p s, S^, p, x); its chain starts from a label y0 drawn
+// from p(y|x) by the posterior kernel and h0 ~ S_{y0}; its negative phase is the last sweep of the same chain with weight beta.
+// The chain runs when alpha > 0 or a row is unlabelled; a batch without an unlabelled row runs exactly the labelled-only step.
+//
+// Draws (Philox, make_rng(seed, site, t, tick, 0)): an unlabelled row's start label SITE_CRBM_Y0 (t = 0); h0 states SITE_H0
+// (t = 0); sweep s = 1..k draws x at SITE_V, the label at SITE_CRBM_Y and h at SITE_H, all with t = s (DESIGN.md §3).
 #pragma once
 
 namespace bm {
@@ -37,11 +42,15 @@ __device__ __forceinline__ float crbm_sigmoid(float x) { return 1.0f / (1.0f + e
 // (a tie goes to the lowest class).  Thread `tid` adds softplus(o[r,y,j]) for j = tid, tid + 256, ... in double; the 256
 // partials of each class are reduced by a fixed xor tree per warp and the 8 warp sums in warp order, so F depends on H alone,
 // never on how many rows a launch has.  U1 is W_1 = U^T [H, C].  CM: classes held in registers (C <= CM).
+// A row labelled -1 (unlabelled) gets no NLL or correctness; instead y0[r] = the label its chain starts from, one categorical
+// draw from the row's float32 p at `yrng` (word 0 of column block 0; the first y whose float64 CDF exceeds u, the CDF formed
+// as dbm_multinomial_rows_kernel forms it).
 template <int CM>
 __global__ void __launch_bounds__(256) crbm_posterior_rows_kernel(const float* __restrict__ A, int H, const float* __restrict__ U1,
                                                                    int C, const float* __restrict__ hb, const float* __restrict__ yb,
                                                                    const int* __restrict__ labels, float* __restrict__ P,
-                                                                   double* __restrict__ nll, int* __restrict__ correct) {
+                                                                   double* __restrict__ nll, int* __restrict__ correct,
+                                                                   RngKey yrng, int* __restrict__ y0) {
     const int r = blockIdx.x, tid = threadIdx.x;
     double acc[CM];
 #pragma unroll
@@ -84,6 +93,21 @@ __global__ void __launch_bounds__(256) crbm_posterior_rows_kernel(const float* _
     for (int y = 0; y < CM; ++y) { if (y >= C) break; P[(size_t)r * C + y] = (float)exp(F[y] - logz); }
     if (labels) {
         const int t = labels[r];
+        if (t < 0) {
+            const float* pr = P + (size_t)r * C;
+            double tot = 0.0, last = 0.0;
+            for (int y = 0; y < C; ++y) tot += (double)pr[y];
+            for (int y = 0; y < C; ++y) last += (double)(float)((double)pr[y] / tot);
+            const double u = (double)u32_to_unit_float(site_block(yrng, (uint32_t)r, 0u).x);
+            double run = 0.0;
+            int pick = C - 1;
+            for (int y = 0; y < C; ++y) {
+                run += (double)(float)((double)pr[y] / tot);
+                if (run / last > u) { pick = y; break; }
+            }
+            y0[r] = pick;
+            return;
+        }
         double Ft = 0.0;
 #pragma unroll
         for (int y = 0; y < CM; ++y) if (y == t) Ft = F[y];
@@ -100,14 +124,17 @@ __global__ void __launch_bounds__(256) crbm_posterior_rows_kernel(const float* _
 //   gU [s, y, j] = sum_r ((1 + alpha) [y == t_r] - p[r, y]) s[r, y, j]
 //   ghb[s, j]  = sum_r G (fp32, before rounding)
 //   gyb[s, y]  = sum_r ((1 + alpha) [y == t_r] - p[r, y])            (block column 0 only)
-// The sums run over the split's rows in order, in fp32.
+// The sums run over the split's rows in order, in fp32.  A row labelled -1 (unlabelled; y0 given) takes the semi-supervised
+// terms with weight beta instead: G = bf16(beta S^), gU += beta p[r, y] s[r, y, j], gyb += beta p[r, y], and its h0 comes
+// from S_{y0[r]}, the label drawn by the posterior kernel.
 template <int CM>
 __global__ void __launch_bounds__(CRBM_COLS) crbm_columns_kernel(const float* __restrict__ A, int H, const float* __restrict__ U1, int C,
                                                                  const float* __restrict__ hb, const float* __restrict__ P,
                                                                  const int* __restrict__ labels, int rows, int rps, float alpha,
                                                                  bf16_t* __restrict__ G, int ldg, bf16_t* __restrict__ h0, int ldh,
                                                                  int sample_h, RngKey rng, float* __restrict__ Sh,
-                                                                 float* __restrict__ gU, float* __restrict__ ghb, float* __restrict__ gyb) {
+                                                                 float* __restrict__ gU, float* __restrict__ ghb, float* __restrict__ gyb,
+                                                                 const int* __restrict__ y0, float beta) {
     const int j = blockIdx.x * CRBM_COLS + threadIdx.x, s = blockIdx.y;
     const int r0 = s * rps, r1 = min(rows, r0 + rps);
     const bool col = j < H;
@@ -121,6 +148,8 @@ __global__ void __launch_bounds__(CRBM_COLS) crbm_columns_kernel(const float* __
     for (int r = r0; r < r1; ++r) {
         const float* pr = P + (size_t)r * C;
         const int t = labels ? labels[r] : -1;
+        const bool unl = y0 && t < 0;
+        const int ts = unl ? y0[r] : t;                   // the label the chain starts from
         if (col) {
             const float a = A[(size_t)r * H + j] + b;
             float sh = 0.f, st = 0.f;
@@ -129,12 +158,12 @@ __global__ void __launch_bounds__(CRBM_COLS) crbm_columns_kernel(const float* __
                 if (y >= C) break;
                 const float sy = crbm_sigmoid(a + u[y]);
                 sh += pr[y] * sy;
-                if (y == t) st = sy;
-                if (gU) gu[y] += ((y == t ? pos : 0.f) - pr[y]) * sy;
+                if (y == ts) st = sy;
+                if (gU) gu[y] += (unl ? beta * pr[y] : (y == t ? pos : 0.f) - pr[y]) * sy;
             }
             if (Sh) Sh[(size_t)r * H + j] = sh;
             if (G) {
-                const float g = pos * st - sh;
+                const float g = unl ? beta * sh : pos * st - sh;
                 G[(size_t)r * ldg + j] = __float2bfloat16_rn(g);
                 hsum += g;
             }
@@ -148,7 +177,7 @@ __global__ void __launch_bounds__(CRBM_COLS) crbm_columns_kernel(const float* __
                 h0[(size_t)r * ldh + j] = __float2bfloat16_rn(h);
             }
         }
-        if (ycol) ysum += ((int)threadIdx.x == t ? pos : 0.f) - pr[threadIdx.x];
+        if (ycol) ysum += unl ? beta * pr[threadIdx.x] : ((int)threadIdx.x == t ? pos : 0.f) - pr[threadIdx.x];
     }
     if (col && gU) {
 #pragma unroll
@@ -158,30 +187,32 @@ __global__ void __launch_bounds__(CRBM_COLS) crbm_columns_kernel(const float* __
     if (ycol) gyb[(size_t)s * C + threadIdx.x] = ysum;
 }
 
-// After the chain (alpha > 0), over the rows of split s = blockIdx.y, thread column j:
-//   aH [r, j]  = bf16(alpha H_k)                                      the negated second pair's operand (ldh)
+// After the chain, over the rows of split s = blockIdx.y, thread column j:
+//   aH [r, j]  = bf16(w_r H_k)                                        the negated second pair's operand (ldh)
 //   yh [s, y, j] = sum_r Y_k[r, y] H_k[r, j]      hk[s, j] = sum_r H_k[r, j]          (j < H)
 //   xd [s, j]  = sum_r X[r, j] - X_k[r, j]                                             (j < V)
 //   yk [s, y]  = sum_r Y_k[r, y]                                                       (block column 0)
+// The sums of pass 0 run over the labelled rows (w_r = alpha) into yh, hk, xd, yk; when yh_u is given, pass 1 runs over the
+// unlabelled rows (label -1, w_r = beta) into yh_u, hk_u, xd_u, yk_u.  Without unlabelled rows pass 0 adds every row in order.
+// one pass: the rows of [r0, r1) whose label is (unl ? -1 : not -1), or every row when labels is null
 template <int CM>
-__global__ void __launch_bounds__(CRBM_COLS) crbm_chain_stats_kernel(const bf16_t* __restrict__ Hk, int ldh, const bf16_t* __restrict__ Yk,
-                                                                     int ldy, int C, const bf16_t* __restrict__ X, const bf16_t* __restrict__ Xk,
-                                                                     int ldx, int V, int H, int rows, int rps, float alpha,
-                                                                     bf16_t* __restrict__ aH, float* __restrict__ yh, float* __restrict__ hk,
-                                                                     float* __restrict__ xd, float* __restrict__ yk) {
-    const int j = blockIdx.x * CRBM_COLS + threadIdx.x, s = blockIdx.y;
-    const int r0 = s * rps, r1 = min(rows, r0 + rps);
+__device__ __forceinline__ void crbm_chain_stats_pass(const bf16_t* __restrict__ Hk, int ldh, const bf16_t* __restrict__ Yk, int ldy,
+                                                      int C, const bf16_t* __restrict__ X, const bf16_t* __restrict__ Xk, int ldx,
+                                                      int V, int H, int r0, int r1, int s, int j, const int* __restrict__ labels,
+                                                      bool unl, float w, bf16_t* __restrict__ aH, float* __restrict__ yh,
+                                                      float* __restrict__ hk, float* __restrict__ xd, float* __restrict__ yk) {
     const bool hcol = j < H, xcol = j < V, ycol = blockIdx.x == 0 && (int)threadIdx.x < C;
     float acc[CM];
 #pragma unroll
     for (int y = 0; y < CM; ++y) acc[y] = 0.f;
     float hs = 0.f, xs = 0.f, ys = 0.f;
     for (int r = r0; r < r1; ++r) {
+        if (labels && (labels[r] < 0) != unl) continue;
         const bf16_t* yr = Yk + (size_t)r * ldy;
         if (hcol) {
             const float h = __bfloat162float(Hk[(size_t)r * ldh + j]);
             hs += h;
-            aH[(size_t)r * ldh + j] = __float2bfloat16_rn(alpha * h);
+            aH[(size_t)r * ldh + j] = __float2bfloat16_rn(w * h);
 #pragma unroll
             for (int y = 0; y < CM; ++y) { if (y >= C) break; acc[y] += __bfloat162float(yr[y]) * h; }
         }
@@ -196,10 +227,28 @@ __global__ void __launch_bounds__(CRBM_COLS) crbm_chain_stats_kernel(const bf16_
     if (xcol) xd[(size_t)s * V + j] = xs;
     if (ycol) yk[(size_t)s * C + threadIdx.x] = ys;
 }
+template <int CM>
+__global__ void __launch_bounds__(CRBM_COLS) crbm_chain_stats_kernel(const bf16_t* __restrict__ Hk, int ldh, const bf16_t* __restrict__ Yk,
+                                                                     int ldy, int C, const bf16_t* __restrict__ X, const bf16_t* __restrict__ Xk,
+                                                                     int ldx, int V, int H, int rows, int rps, float alpha,
+                                                                     bf16_t* __restrict__ aH, float* __restrict__ yh, float* __restrict__ hk,
+                                                                     float* __restrict__ xd, float* __restrict__ yk,
+                                                                     const int* __restrict__ labels, float beta, float* __restrict__ yh_u,
+                                                                     float* __restrict__ hk_u, float* __restrict__ xd_u, float* __restrict__ yk_u) {
+    const int j = blockIdx.x * CRBM_COLS + threadIdx.x, s = blockIdx.y;
+    const int r0 = s * rps, r1 = min(rows, r0 + rps);
+    if (!yh_u) {            // every row labelled: one pass over all of them
+        crbm_chain_stats_pass<CM>(Hk, ldh, Yk, ldy, C, X, Xk, ldx, V, H, r0, r1, s, j, nullptr, false, alpha, aH, yh, hk, xd, yk);
+        return;
+    }
+    crbm_chain_stats_pass<CM>(Hk, ldh, Yk, ldy, C, X, Xk, ldx, V, H, r0, r1, s, j, labels, false, alpha, aH, yh, hk, xd, yk);
+    crbm_chain_stats_pass<CM>(Hk, ldh, Yk, ldy, C, X, Xk, ldx, V, H, r0, r1, s, j, labels, true, beta, aH, yh_u, hk_u, xd_u, yk_u);
+}
 
 // The hybrid step's update of every variable (one thread per element of [W | U | vb | hb | yb]):
 //   grad = (disc + alpha gen sums) / N  [- l2 theta for W and U];   d = lr (mom d + grad);   theta += d;  bf16 shadows refreshed.
-// Sums over s1 split-K slices (W) or s2 / s3 row splits; the gen-only terms are read when s3 > 0.
+// Sums over s1 split-K slices (W) or s2 / s3 / s4 row splits; the gen-only terms are read when s3 > 0, and the unlabelled
+// rows' chain statistics (weight beta, yhu / hku / xdu / yku) when s4 > 0.
 struct CrbmUpdate {
     int V, H, C, ld1, ld2;
     float *W, *dW, *U1, *dU1, *vb, *dvb, *hb, *dhb, *yb, *dyb;
@@ -208,7 +257,14 @@ struct CrbmUpdate {
     const float *gU, *ghb, *gyb; int s2;
     const float *yh, *hk, *xd, *yk; int s3;
     float alpha, N, l2, lr, mom;
+    const float *yhu, *hku, *xdu, *yku; int s4;
+    float beta;
 };
+__device__ __forceinline__ float crbm_split_sum(const float* p, int n, size_t stride, size_t i) {
+    float b = 0.f;
+    for (int s = 0; s < n; ++s) b += p[(size_t)s * stride + i];
+    return b;
+}
 __global__ void crbm_update_kernel(CrbmUpdate u) {
     const size_t nW = (size_t)u.V * u.H, nU = (size_t)u.C * u.H;
     const size_t n = nW + nU + u.V + u.H + u.C;
@@ -226,27 +282,35 @@ __global__ void crbm_update_kernel(CrbmUpdate u) {
             for (int s = 0; s < u.s2; ++s) a += u.gU[(size_t)s * nU + k];
             for (int s = 0; s < u.s3; ++s) b += u.yh[(size_t)s * nU + k];
             th = u.U1 + (size_t)j * u.C + y; d = u.dU1 + (size_t)j * u.C + y;
-            g = (a - u.alpha * b) / u.N - u.l2 * *th;
+            float c = a - u.alpha * b;
+            if (u.s4) c -= u.beta * crbm_split_sum(u.yhu, u.s4, nU, k);
+            g = c / u.N - u.l2 * *th;
         } else if (i < nW + nU + u.V) {
             const int j = (int)(i - nW - nU);
             float b = 0.f;
             for (int s = 0; s < u.s3; ++s) b += u.xd[(size_t)s * u.V + j];
             th = u.vb + j; d = u.dvb + j;
-            g = u.alpha * b / u.N;
+            float c = u.alpha * b;
+            if (u.s4) c += u.beta * crbm_split_sum(u.xdu, u.s4, u.V, j);
+            g = c / u.N;
         } else if (i < nW + nU + u.V + u.H) {
             const int j = (int)(i - nW - nU - u.V);
             float a = 0.f, b = 0.f;
             for (int s = 0; s < u.s2; ++s) a += u.ghb[(size_t)s * u.H + j];
             for (int s = 0; s < u.s3; ++s) b += u.hk[(size_t)s * u.H + j];
             th = u.hb + j; d = u.dhb + j;
-            g = (a - u.alpha * b) / u.N;
+            float c = a - u.alpha * b;
+            if (u.s4) c -= u.beta * crbm_split_sum(u.hku, u.s4, u.H, j);
+            g = c / u.N;
         } else {
             const int y = (int)(i - nW - nU - u.V - u.H);
             float a = 0.f, b = 0.f;
             for (int s = 0; s < u.s2; ++s) a += u.gyb[(size_t)s * u.C + y];
             for (int s = 0; s < u.s3; ++s) b += u.yk[(size_t)s * u.C + y];
             th = u.yb + y; d = u.dyb + y;
-            g = (a - u.alpha * b) / u.N;
+            float c = a - u.alpha * b;
+            if (u.s4) c -= u.beta * crbm_split_sum(u.yku, u.s4, u.C, y);
+            g = c / u.N;
         }
         const float dd = u.lr * (u.mom * *d + g);
         *d = dd;
@@ -287,11 +351,11 @@ struct CrbmShape {       // the arrays a bm_dbm_cfg points into, alive while Dbm
 // ---------------------------------------------------------------------------------------------
 struct ClassRbmTC : DbmTC {
     int C, H;
-    float alpha;
+    float alpha, beta;
     int smp_v, smp_h;
     DevBuf<float> A, P, Sh, part;
     DevBuf<double> nll;
-    DevBuf<int> correct, lab;
+    DevBuf<int> correct, lab, y0;
     DevBuf<bf16_t> Gb, aHb;
 
     // refusals name the option (BM_EUNSUPPORTED); shapes and classes are BM_EINVAL
@@ -299,6 +363,7 @@ struct ClassRbmTC : DbmTC {
         BM_REQUIRE(f.n_visible > 0 && f.n_hidden > 0 && f.max_batch > 0, "bad classification RBM shape");
         BM_REQUIRE(f.n_classes >= CRBM_MIN_CLASSES && f.n_classes <= CRBM_MAX_CLASSES, "n_classes must be in [2, 64]");
         BM_REQUIRE(f.alpha >= 0.0, "alpha must be non-negative");
+        BM_REQUIRE(f.beta >= 0.0 && std::isfinite(f.beta), "beta must be finite and non-negative");
         if (f.dtype != BM_DTYPE_F32) throw Error(BM_EUNSUPPORTED, "classification RBMs support float32 models only (dtype float64 requested)");
         if (f.compute != BM_COMPUTE_BF16) throw Error(BM_EUNSUPPORTED, "classification RBMs run on the tensor-core engine only (compute fp32 requested)");
         if (f.dropout_keep >= 0.0) throw Error(BM_EUNSUPPORTED, "classification RBMs do not support dropout");
@@ -308,9 +373,9 @@ struct ClassRbmTC : DbmTC {
     }
     ClassRbmTC(Ctx* c, const bm_crbm_cfg& f, CrbmShape& s)
         : DbmTC(c, crbm_as_dbm(f, s.Hs, s.kinds, s.ns, s.smp, s.spt, s.spc)) {
-        C = f.n_classes; H = f.n_hidden; alpha = (float)f.alpha; smp_v = f.sample_v; smp_h = f.sample_h;
+        C = f.n_classes; H = f.n_hidden; alpha = (float)f.alpha; beta = (float)f.beta; smp_v = f.sample_v; smp_h = f.sample_h;
         A.ensure((size_t)B * H); P.ensure((size_t)B * C); Sh.ensure((size_t)B * H);
-        nll.ensure(B); correct.ensure(B); lab.ensure(B);
+        nll.ensure(B); correct.ensure(B); lab.ensure(B); y0.ensure(B);
         Gb.ensure((size_t)B * ldn[1]); aHb.ensure((size_t)B * ldn[1]);
         for (DevBuf<bf16_t>* b : {&Gb, &aHb}) b->zero(ctx->stream);
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -366,19 +431,27 @@ struct ClassRbmTC : DbmTC {
     void forward(int rows) {                                   // A = X W (fp32, bias-free)
         linear_tc(Xb.p, ldn[0], rows, V, Wb[0].p, V, H, ldn[1], true, H, nullptr, A.p);
     }
-    void posterior(int rows, const int* labels) {
-        if (C <= 16) crbm_posterior_rows_kernel<16><<<rows, 256, 0, ctx->stream>>>(A.p, H, W[1].p, C, hb[0].p, hb[1].p, labels, P.p, nll.p, correct.p);
-        else crbm_posterior_rows_kernel<64><<<rows, 256, 0, ctx->stream>>>(A.p, H, W[1].p, C, hb[0].p, hb[1].p, labels, P.p, nll.p, correct.p);
+    // yrng: the draw site of the chain's start label for rows labelled -1
+    void posterior(int rows, const int* labels, RngKey yrng = RngKey{}) {
+        if (C <= 16)
+            crbm_posterior_rows_kernel<16><<<rows, 256, 0, ctx->stream>>>(A.p, H, W[1].p, C, hb[0].p, hb[1].p, labels, P.p, nll.p, correct.p,
+                                                                          yrng, y0.p);
+        else
+            crbm_posterior_rows_kernel<64><<<rows, 256, 0, ctx->stream>>>(A.p, H, W[1].p, C, hb[0].p, hb[1].p, labels, P.p, nll.p, correct.p,
+                                                                          yrng, y0.p);
         count_launch(ctx);
     }
-    void columns(int rows, const int* labels, bf16_t* G, bf16_t* h0, RngKey rng, float* sh, float* gU, float* ghb, float* gyb) {
+    // semi: the batch holds rows labelled -1, whose chain starts from y0 (written by `posterior`)
+    void columns(int rows, const int* labels, bf16_t* G, bf16_t* h0, RngKey rng, float* sh, float* gU, float* ghb, float* gyb,
+                 bool semi = false) {
         const dim3 grid((H + CRBM_COLS - 1) / CRBM_COLS, splits(rows));
+        const int* start = semi ? y0.p : nullptr;
         if (C <= 16)
             crbm_columns_kernel<16><<<grid, CRBM_COLS, 0, ctx->stream>>>(A.p, H, W[1].p, C, hb[0].p, P.p, labels, rows, CRBM_ROWS_PER_SPLIT, alpha,
-                                                                         G, ldn[1], h0, ldn[1], smp_h, rng, sh, gU, ghb, gyb);
+                                                                         G, ldn[1], h0, ldn[1], smp_h, rng, sh, gU, ghb, gyb, start, beta);
         else
             crbm_columns_kernel<64><<<grid, CRBM_COLS, 0, ctx->stream>>>(A.p, H, W[1].p, C, hb[0].p, P.p, labels, rows, CRBM_ROWS_PER_SPLIT, alpha,
-                                                                         G, ldn[1], h0, ldn[1], smp_h, rng, sh, gU, ghb, gyb);
+                                                                         G, ldn[1], h0, ldn[1], smp_h, rng, sh, gU, ghb, gyb, start, beta);
         count_launch(ctx);
     }
     void check_rows(int rows) const { BM_REQUIRE(rows >= 1 && rows <= B, "a batch must have 1..max_batch rows"); }
@@ -388,23 +461,30 @@ struct ClassRbmTC : DbmTC {
                     int want, double* out) {
         check_rows(rows);
         BM_REQUIRE(labels, "null labels");
-        for (int r = 0; r < rows; ++r)
-            if (labels[r] < 0 || labels[r] >= C) throw Error(BM_EINVAL, "label " + std::to_string(labels[r]) + " of row " + std::to_string(r) + " is outside [0, n_classes)");
-        const bool gen = alpha > 0.f;
-        BM_REQUIRE(!gen || k >= 1, "n_gibbs_steps must be at least 1 when alpha > 0");
+        int unlabelled = 0;
+        for (int r = 0; r < rows; ++r) {
+            if (labels[r] == -1 && beta > 0.f) { ++unlabelled; continue; }
+            if (labels[r] < 0 || labels[r] >= C)
+                throw Error(BM_EINVAL, "label " + std::to_string(labels[r]) + " of row " + std::to_string(r) + " is outside [0, n_classes)" +
+                                           (labels[r] == -1 ? " (-1 marks an unlabelled row only when beta > 0)" : ""));
+        }
+        const bool semi = unlabelled > 0;
+        const bool gen = alpha > 0.f || semi;                    // the chain runs for the generative terms of either kind
+        BM_REQUIRE(!gen || k >= 1, "n_gibbs_steps must be at least 1 when alpha > 0 or a row is unlabelled");
         BM_REQUIRE(!want || out, "metrics requested without a buffer");
         upload_tc(Xh, rows);
         BM_CUDA(cudaMemcpyAsync(lab.p, labels, (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
         forward(rows);
-        posterior(rows, lab.p);
-        // partials: [W slices | gU | ghb | gyb] then, with the chain, [yh | hk | xd | yk]
-        const int s2 = splits(rows), s3 = gen ? s2 : 0;
+        posterior(rows, lab.p, make_rng(seed, SITE_CRBM_Y0, 0, tick, 0));
+        // partials: [W slices | gU | ghb | gyb] then, with the chain, [yh | hk | xd | yk] and, with unlabelled rows,
+        // [yhu | hku | xdu | yku]
+        const int s2 = splits(rows), s3 = gen ? s2 : 0, s4 = semi ? s2 : 0;
         const int total_pairs = ctx->sm_count / 2;
         const int pair_tiles = ((V + 255) / 256) * ((H + 255) / 256);
         const int s1 = std::max(1, std::min(total_pairs / std::max(pair_tiles, 1), (rows + 63) / 64));
         const size_t wstride = (size_t)V * H, nU = (size_t)C * H;
         const size_t per = nU + H + C, per_gen = nU + H + V + C;
-        part.ensure((size_t)s1 * wstride + (size_t)s2 * per + (size_t)s3 * per_gen);
+        part.ensure((size_t)s1 * wstride + (size_t)s2 * per + (size_t)(s3 + s4) * per_gen);
         float* Wp = part.p;
         float* gU = Wp + (size_t)s1 * wstride;
         float* ghb = gU + (size_t)s2 * nU;
@@ -413,7 +493,11 @@ struct ClassRbmTC : DbmTC {
         float* hk = yh + (size_t)s3 * nU;
         float* xd = hk + (size_t)s3 * H;
         float* yk = xd + (size_t)s3 * V;
-        columns(rows, lab.p, Gb.p, gen ? h_b[0].p : nullptr, make_rng(seed, SITE_H0, 0, tick, 0), nullptr, gU, ghb, gyb);
+        float* yhu = yk + (size_t)s3 * C;
+        float* hku = yhu + (size_t)s4 * nU;
+        float* xdu = hku + (size_t)s4 * H;
+        float* yku = xdu + (size_t)s4 * V;
+        columns(rows, lab.p, Gb.p, gen ? h_b[0].p : nullptr, make_rng(seed, SITE_H0, 0, tick, 0), nullptr, gU, ghb, gyb, semi);
         bf16_t* hc = h_b[0].p;
         if (gen) {
             bf16_t* hn = h2_b[0].p;
@@ -424,12 +508,15 @@ struct ClassRbmTC : DbmTC {
                 std::swap(hc, hn);
             }
             const dim3 grid((std::max(V, H) + CRBM_COLS - 1) / CRBM_COLS, s3);
+            float* const uyh = semi ? yhu : nullptr;
             if (C <= 16)
                 crbm_chain_stats_kernel<16><<<grid, CRBM_COLS, 0, ctx->stream>>>(hc, ldn[1], h_b[1].p, ldn[2], C, Xb.p, v_b.p, ldn[0], V, H, rows,
-                                                                                 CRBM_ROWS_PER_SPLIT, alpha, aHb.p, yh, hk, xd, yk);
+                                                                                 CRBM_ROWS_PER_SPLIT, alpha, aHb.p, yh, hk, xd, yk,
+                                                                                 lab.p, beta, uyh, hku, xdu, yku);
             else
                 crbm_chain_stats_kernel<64><<<grid, CRBM_COLS, 0, ctx->stream>>>(hc, ldn[1], h_b[1].p, ldn[2], C, Xb.p, v_b.p, ldn[0], V, H, rows,
-                                                                                 CRBM_ROWS_PER_SPLIT, alpha, aHb.p, yh, hk, xd, yk);
+                                                                                 CRBM_ROWS_PER_SPLIT, alpha, aHb.p, yh, hk, xd, yk,
+                                                                                 lab.p, beta, uyh, hku, xdu, yku);
             count_launch(ctx);
         }
         {   // X^T G [- X_k^T (alpha H_k)]: one split-K op over the batch rows
@@ -448,15 +535,16 @@ struct ClassRbmTC : DbmTC {
             g.out_f32 = Wp; g.ld_f32 = H;
             launch_tc_gemm(ctx, g);
         }
-        if (want) {         // the pre-update posterior of this batch
+        if (want) {         // the pre-update posterior of this batch's labelled rows (NaN for a batch without one)
             std::vector<double> hn(rows);
             std::vector<int> hc_(rows);
             BM_CUDA(cudaMemcpyAsync(hn.data(), nll.p, (size_t)rows * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
             BM_CUDA(cudaMemcpyAsync(hc_.data(), correct.p, (size_t)rows * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
             BM_CUDA(cudaStreamSynchronize(ctx->stream));
             double a = 0.0, c = 0.0;
-            for (int r = 0; r < rows; ++r) { a += hn[r]; c += hc_[r]; }
-            out[0] = a / rows; out[1] = c / rows;
+            for (int r = 0; r < rows; ++r) if (labels[r] >= 0) { a += hn[r]; c += hc_[r]; }
+            const int n = rows - unlabelled;
+            out[0] = n ? a / n : std::nan(""); out[1] = n ? c / n : std::nan("");
         }
         CrbmUpdate u;
         u.V = V; u.H = H; u.C = C; u.ld1 = ldn[1]; u.ld2 = ldn[2];
@@ -467,6 +555,7 @@ struct ClassRbmTC : DbmTC {
         u.gU = gU; u.ghb = ghb; u.gyb = gyb; u.s2 = s2;
         u.yh = yh; u.hk = hk; u.xd = xd; u.yk = yk; u.s3 = s3;
         u.alpha = alpha; u.N = (float)rows; u.l2 = (float)l2; u.lr = (float)lr; u.mom = (float)mom;
+        u.yhu = yhu; u.hku = hku; u.xdu = xdu; u.yku = yku; u.s4 = s4; u.beta = beta;
         const size_t n = wstride + nU + V + H + C;
         crbm_update_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, 4096), 256, 0, ctx->stream>>>(u);
         count_launch(ctx);

@@ -286,6 +286,8 @@ typedef struct bm_crbm_cfg {
     double  dropout_keep;            /* < 0 (none); anything else is refused */
     double  sparsity_cost;           /* 0; anything else is refused */
     int32_t dbm_first, dbm_last;     /* 0; anything else is refused */
+    double  beta;                    /* weight of beta * CD-k of log p(x) for rows labelled -1 (semi-supervised, Larochelle
+                                        et al., JMLR 2012); 0 (the default) refuses -1; negative or non-finite: BM_EINVAL */
 } bm_crbm_cfg;
 int  bm_crbm_create(bm_ctx* ctx, const bm_crbm_cfg* cfg, bm_crbm** out);
 void bm_crbm_destroy(bm_crbm* crbm);
@@ -295,7 +297,11 @@ int  bm_crbm_get_param(bm_crbm* crbm, const char* name, void* host, size_t bytes
 /* W <- N(0, stddev) from tf.random_normal's stream of op_seed_w, U [C,H] likewise from op_seed_u */
 int  bm_crbm_init_weights(bm_crbm* crbm, double stddev, uint64_t op_seed_w, uint64_t op_seed_u);
 /* one hybrid step on X [rows, n_visible] (float32) with labels [rows] in [0, n_classes) (BM_EINVAL before any launch
- * otherwise); 1 <= rows <= max_batch.  want_metrics != 0: out2 = {mean -log p(t|x), accuracy} under the pre-update weights */
+ * otherwise); 1 <= rows <= max_batch.  With beta > 0 a label of -1 marks an unlabelled row: it adds beta * CD-k of log p(x)
+ * (exact positive phase; the chain starts from a label drawn from p(y|x)) and the chain runs even at alpha = 0; with
+ * beta = 0, -1 is refused like any label outside [0, n_classes).  A batch without -1 computes what it computes at beta = 0.
+ * want_metrics != 0: out2 = {mean -log p(t|x), accuracy} over the labelled rows under the pre-update weights (NaN, NaN
+ * when the batch has none) */
 int  bm_crbm_train_step(bm_crbm* crbm, const void* X, const int32_t* labels, int32_t rows, double lr, double momentum,
                         int32_t n_gibbs_steps, uint64_t seed, uint32_t tick, int32_t want_metrics, double* out2);
 int  bm_crbm_predict_proba(bm_crbm* crbm, const void* X, int32_t rows, float* out);    /* p(y|x): out [rows, n_classes] */
