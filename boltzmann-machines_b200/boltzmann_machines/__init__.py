@@ -8,6 +8,6 @@ from . import utils
 from . import layers
 from . import ebm
 from . import rbm
-from .rbm import BaseRBM, BernoulliRBM, MultinomialRBM, GaussianRBM, ClassificationRBM, logit_mean
+from .rbm import BaseRBM, BernoulliRBM, MultinomialRBM, GaussianRBM, ClassificationRBM, logit_mean, fit_many
 from . import dbm
 from .dbm import DBM

@@ -33,6 +33,8 @@ EXPORTS = (
     'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows', 'bm_debug_dbm_multinomial_rows',
     'bm_crbm_create', 'bm_crbm_destroy', 'bm_crbm_set_param', 'bm_crbm_get_param', 'bm_crbm_init_weights',
     'bm_crbm_train_step', 'bm_crbm_predict_proba', 'bm_crbm_transform',
+    'bm_rbm_group_create', 'bm_rbm_group_destroy', 'bm_rbm_group_train_epoch', 'bm_rbm_group_train_epoch_u8',
+    'bm_rbm_group_train_epoch_bf16',
 )
 
 
@@ -163,7 +165,11 @@ def load_library(path=None):
         'bm_crbm_init_weights': [vp, dbl, u64, u64],
         'bm_crbm_train_step': [vp, vp, vp, i32, dbl, dbl, i32, u64, u32, i32, C.POINTER(dbl)],
         'bm_crbm_predict_proba': [vp, vp, i32, vp], 'bm_crbm_transform': [vp, vp, i32, vp],
+        'bm_rbm_group_create': [vp, vp, i32, C.POINTER(vp)],
     }
+    group_epoch = [vp, vp, i64, i32, vp, vp, i32, vp, vp, vp, vp, vp, vp]
+    for name in ('bm_rbm_group_train_epoch', 'bm_rbm_group_train_epoch_u8', 'bm_rbm_group_train_epoch_bf16'):
+        protos[name] = group_epoch
     for name, argtypes in protos.items():
         fn = getattr(lib, name)
         fn.argtypes = argtypes
@@ -176,6 +182,8 @@ def load_library(path=None):
     lib.bm_dbm_destroy.restype = None
     lib.bm_crbm_destroy.argtypes = [vp]
     lib.bm_crbm_destroy.restype = None
+    lib.bm_rbm_group_destroy.argtypes = [vp]
+    lib.bm_rbm_group_destroy.restype = None
     if path is None:
         _lib = lib
     return lib
@@ -577,12 +585,16 @@ class CudaRBM(object):
         if as_bytes(X, out=P) is not None:
             return P
         pinned_free(P)
-        # real-valued data: the bf16 engine rounds its input to bfloat16 before the first GEMM, so feeding the rounded
-        # values is bit-identical and halves the copy (not with dropout / sigma scaling, which act on the fp32 input first)
-        if (self.compute == 'bf16' and self.dt == np.float32 and self.cfg.get('v_kind', 'bernoulli') == 'bernoulli' and
-                self.cfg.get('h_kind', 'bernoulli') == 'bernoulli' and self.cfg.get('dropout') is None):
+        if self.feeds_bf16():
             return as_bf16(X, out=pinned_empty(X.shape, np.uint16))
         return pinned_copy(X)
+
+    def feeds_bf16(self):
+        """Whether real-valued training data goes to this engine as bfloat16: the bf16 engine rounds its input to bfloat16
+        before the first GEMM, so feeding the rounded values is bit-identical and halves the copy (not with dropout / sigma
+        scaling, which act on the fp32 input first)."""
+        return (self.compute == 'bf16' and self.dt == np.float32 and self.cfg.get('v_kind', 'bernoulli') == 'bernoulli' and
+                self.cfg.get('h_kind', 'bernoulli') == 'bernoulli' and self.cfg.get('dropout') is None)
 
     def unpin(self, P):
         pinned_free(np.asarray(P))
@@ -636,6 +648,77 @@ class CudaRBM(object):
     def close(self):
         if getattr(self, 'handle', None):
             self._lib.bm_rbm_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class CudaRBMGroup(object):
+    """Engine object for ``fit_many``: a ``bm_rbm_group`` handle over CudaRBM engines of one shape, which stay usable on
+    their own.  Refused engine options raise NotImplementedError."""
+
+    def __init__(self, engines):
+        self._lib = load_library()
+        self.engines = list(engines)
+        n = len(self.engines)
+        handles = (C.c_void_p * n)(*[e.handle.value for e in self.engines])
+        h = C.c_void_p()
+        self._check(self._lib.bm_rbm_group_create(self.engines[0].ctx.handle, handles, n, C.byref(h)))
+        self.handle = h
+
+    def _check(self, rc):
+        if rc == -5:                                        # BM_EUNSUPPORTED
+            raise NotImplementedError(self._lib.bm_last_error().decode('utf-8', 'replace'))
+        check(rc)
+
+    def pin(self, Xs):
+        """The members' training sets [n, rows, n_visible] in page-locked memory, in the format each member's own `pin` would
+        feed with the same values: bytes when every value is an integer in 0..255, bfloat16 for engines that round their input
+        to it anyway, float32 otherwise."""
+        X = np.ascontiguousarray(np.stack([e._batch(x) for e, x in zip(self.engines, Xs)]))
+        P = pinned_empty(X.shape, np.uint8)
+        if as_bytes(X, out=P) is not None:
+            return P
+        pinned_free(P)
+        if all(e.feeds_bf16() for e in self.engines):
+            return as_bf16(X, out=pinned_empty(X.shape, np.uint16))
+        return pinned_copy(X)
+
+    def unpin(self, P):
+        pinned_free(np.asarray(P))
+
+    def train_epoch(self, X, batch, lr, momentum, k, seed, tick0, metrics, every, iter0):
+        """One epoch of every member: member m trains on X[m] exactly as engines[m].train_epoch(X[m], batch, lr[m], ...) would.
+        Per-member lists: lr, momentum, seed, tick0, metrics (names), every, iter0.  Returns one {metric: [values]} per member."""
+        n = len(self.engines)
+        byte_valued = X.dtype == np.uint8 and not isinstance(X, Bf16Array)
+        fn = (self._lib.bm_rbm_group_train_epoch_u8 if byte_valued else
+              self._lib.bm_rbm_group_train_epoch_bf16 if isinstance(X, Bf16Array) else self._lib.bm_rbm_group_train_epoch)
+        if X.ndim != 3 or X.shape[0] != n or X.shape[2] != self.engines[0].V or not X.flags['C_CONTIGUOUS']:
+            raise ValueError('training sets have shape {0}, expected ({1}, rows, {2})'.format(X.shape, n, self.engines[0].V))
+        nb = (X.shape[1] + batch - 1) // batch
+        out = np.zeros((n, nb, 4), dtype=np.float64)
+        arr = lambda v, dt: np.ascontiguousarray(v, dtype=dt)
+        lr, momentum = arr(lr, np.float64), arr(momentum, np.float64)
+        seeds = arr([int(s) & (2 ** 64 - 1) for s in seed], np.uint64)
+        ticks, masks = arr(tick0, np.uint32), arr([_mask(m) for m in metrics], np.uint32)
+        every, iter0 = arr(every, np.int32), arr(iter0, np.int64)
+        self._check(fn(self.handle, X.ctypes.data, X.shape[1], int(batch), lr.ctypes.data, momentum.ctypes.data, int(k),
+                       seeds.ctypes.data, ticks.ctypes.data, masks.ctypes.data, every.ctypes.data, iter0.ctypes.data,
+                       out.ctypes.data))
+        res = []
+        for g in range(n):
+            rep = [i for i in range(nb) if every[g] and (iter0[g] + i + 1) % every[g] == 0]
+            res.append({m: [float(out[g, i, METRIC_SLOTS[m]]) for i in rep] for m in metrics[g]})
+        return res
+
+    def close(self):
+        if getattr(self, 'handle', None):
+            self._lib.bm_rbm_group_destroy(self.handle)
             self.handle = None
 
     def __del__(self):
@@ -893,4 +976,6 @@ def default_factory(kind):
         return CudaRBM
     if kind == 'crbm':
         return CudaCRBM
+    if kind == 'rbm_group':
+        return CudaRBMGroup
     raise RuntimeError("no native engine for '{0}'".format(kind))

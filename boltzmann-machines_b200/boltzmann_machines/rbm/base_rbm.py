@@ -235,13 +235,7 @@ class BaseRBM(EnergyBasedModel):
                                                 metrics=wanted, every=every or 0, iter0=self.iter_ + b0, **self._step_args())
                 for m in wanted:
                     got[m].extend(part[m])
-            self._tick += len(bounds)
-            if every:
-                steps = [self.iter_ + i + 1 for i in range(len(bounds)) if (self.iter_ + i + 1) % every == 0]
-                for j, step in enumerate(steps):
-                    self._log_scalars('train', step, {self._METRIC_TAGS[m]: got[m][j] for m in wanted}, allow_empty=True)
-            self.iter_ += len(bounds)
-            return {m: (float(np.mean(got[m])) if got[m] else None) for m in wanted}
+            return self._log_train_epoch(got, len(bounds))
         for lo, hi in _maybe_bar(bounds, self.verbose, leave=False, ncols=64, desc='epoch'):
             self.iter_ += 1
             reporting = bool(every and self.iter_ % every == 0)
@@ -255,6 +249,18 @@ class BaseRBM(EnergyBasedModel):
                 # train metric is enabled (base_rbm.py:554-564)
                 self._log_scalars('train', self.iter_, {self._METRIC_TAGS[m]: got[m] for m in report}, allow_empty=True)
         return {m: (float(np.mean(v)) if v else None) for m, v in sums.items()}
+
+    def _log_train_epoch(self, got, n_batches):
+        """Bookkeeping of an epoch the engine ran in one go: ticks, iterations and the train scalars of the reporting batches
+        (`got`: {metric: [value of every reporting batch]}).  Returns the epoch's mean of every metric."""
+        every = self.metrics_config['train_metrics_every_iter']
+        self._tick += n_batches
+        if every:
+            steps = [self.iter_ + i + 1 for i in range(n_batches) if (self.iter_ + i + 1) % every == 0]
+            for j, step in enumerate(steps):
+                self._log_scalars('train', step, {self._METRIC_TAGS[m]: got[m][j] for m in got}, allow_empty=True)
+        self.iter_ += n_batches
+        return {m: (float(np.mean(v)) if v else None) for m, v in got.items()}
 
     def _run_val_metrics(self, X_val):
         wanted = self._enabled(self._VAL_METRICS)
@@ -293,35 +299,38 @@ class BaseRBM(EnergyBasedModel):
         X = np.ascontiguousarray(X, dtype=self._np_dtype)
         if X_val is not None:
             X_val = np.ascontiguousarray(X_val, dtype=self._np_dtype)
-        mc = self.metrics_config
         pinned = self._engine.pin(X) if hasattr(self._engine, 'pin') else None   # page-locked copy: async uploads
         if pinned is not None:
             X = pinned
         try:
             for self.epoch_ in epoch_iter(start_epoch=self.epoch_, max_epoch=self.max_epoch,
                                           verbose=self.verbose):
-                train_results = self._train_epoch(X)
-                val_results, feg = {}, None
-                if X_val is not None and self.epoch_ % mc['val_metrics_every_epoch'] == 0:
-                    val_results = self._run_val_metrics(X_val)
-                if X_val is not None and mc['feg'] and self.epoch_ % mc['feg_every_epoch'] == 0:
-                    feg = self._run_feg(X, X_val)
-
-                if self.verbose:
-                    line = 'epoch: {0:{1}}/{2}'.format(self.epoch_, len(str(self.max_epoch)), self.max_epoch)
-                    for prefix, res in (('', train_results), ('val.', val_results)):
-                        for m in sorted(res):
-                            if res[m] is not None:
-                                line += '; {0}{1}: {2:{3}}'.format(prefix, m, res[m], mc[m + '_fmt'])
-                    if feg is not None:
-                        line += ' ; feg: {0:{1}}'.format(feg, mc['feg_fmt'])
-                    write_during_training(line)
-
-                if self.save_after_each_epoch:
-                    self._save_model(global_step=self.epoch_)
+                self._end_epoch(X, X_val, self._train_epoch(X))
         finally:
             if pinned is not None:
                 self._engine.unpin(pinned)
+
+    def _end_epoch(self, X, X_val, train_results):
+        """What follows the training batches of an epoch: validation metrics, free-energy gap, verbose line, checkpoint."""
+        mc = self.metrics_config
+        val_results, feg = {}, None
+        if X_val is not None and self.epoch_ % mc['val_metrics_every_epoch'] == 0:
+            val_results = self._run_val_metrics(X_val)
+        if X_val is not None and mc['feg'] and self.epoch_ % mc['feg_every_epoch'] == 0:
+            feg = self._run_feg(X, X_val)
+
+        if self.verbose:
+            line = 'epoch: {0:{1}}/{2}'.format(self.epoch_, len(str(self.max_epoch)), self.max_epoch)
+            for prefix, res in (('', train_results), ('val.', val_results)):
+                for m in sorted(res):
+                    if res[m] is not None:
+                        line += '; {0}{1}: {2:{3}}'.format(prefix, m, res[m], mc[m + '_fmt'])
+            if feg is not None:
+                line += ' ; feg: {0:{1}}'.format(feg, mc['feg_fmt'])
+            write_during_training(line)
+
+        if self.save_after_each_epoch:
+            self._save_model(global_step=self.epoch_)
 
     def init_from(self, rbm):
         """Start from another RBM's weights, momentum accumulators and

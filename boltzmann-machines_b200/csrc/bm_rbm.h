@@ -26,6 +26,24 @@ struct DevBuf {
 
 enum : int { SRC_NATIVE = 0, SRC_U8 = 1, SRC_BF16 = 2 };
 
+// What a training group (bm_rbm_group.cu) asks of a tensor-core model: the group runs the training steps of several models
+// of one shape in shared program launches and updates them all in one launch.
+struct TcGroupMember {
+    virtual ~TcGroupMember() {}
+    // builds the program of one training step exactly as the model's own step does, reading the batch from rows
+    // [base, base + rows) of the bf16 input X (ld, rows_total rows) shifted by the launch's batch cursor `cursor`; Xf holds the
+    // same rows in fp32 for the metrics.  The model's activations then describe this step.
+    virtual TcProgram& group_step(const __nv_bfloat16* X, int ld, int rows_total, int base, int cursor, const float* Xf, int rows,
+                                  int k) = 0;
+    virtual CdTail group_tail(int rows, double lr, double mom) const = 0;     // the update of that step
+    virtual void group_step_done() = 0;                                         // after the update was queued
+    virtual std::vector<bm_tc_op_plan>& group_plan() = 0;                       // what bm_rbm_debug_tc_plan reports
+    // the metrics of `mask` under the step's pre-update weights, read back asynchronously into dst[8] ...
+    virtual void group_metrics(uint32_t mask, int rows, uint64_t seed, uint32_t tick, double* dst) = 0;
+    // ... and turned into the four slots of bm_rbm_train_epoch once the stream has been synchronised
+    virtual void group_finish_metrics(const double* h, uint32_t mask, double* out) const = 0;
+};
+
 struct RbmBase {
     Ctx* ctx = nullptr;
     bm_rbm_cfg cfg{};
@@ -45,6 +63,7 @@ struct RbmBase {
     virtual void get_activation(const char* name, void* host, size_t bytes) = 0;
     // test hook (bm_rbm_debug_tc_plan): the ops of the last tensor-core program
     virtual const std::vector<bm_tc_op_plan>& tc_plan() const { throw Error(BM_EINVAL, "this engine runs no tensor-core program"); }
+    virtual TcGroupMember* tc_group_member() { return nullptr; }       // null: the engine cannot train in a group
 };
 
 // ------------------------------------------------------------------------------------------

@@ -18,7 +18,7 @@ namespace bm {
 
 static inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
-struct RbmTC : RbmSimt<float> {
+struct RbmTC : RbmSimt<float>, TcGroupMember {
     typedef __nv_bfloat16 bf16;
     int ldw, ldv, ldh;
     DevBuf<bf16> Wb, Xb, h0m_b, h0s_b, vm_b, vs_b, hm_b, hs_b, data_b;
@@ -28,7 +28,9 @@ struct RbmTC : RbmSimt<float> {
     bool tc_kinds;
     // state of the last chain
     const bf16* X_b = nullptr; int X_ld = 0; int X_row0 = 0; int X_rows_total = 0;
-    int X_mode = 0;       // 0: a buffer of exactly this batch; 1: rows [X_row0, ..) of the resident dataset; 2: a half of the epoch double buffer (1, 2: the program takes the row as its batch cursor)
+    int X_mode = 0;       // 0: a buffer of exactly this batch; 1: rows [X_row0, ..) of the resident dataset; 2: a half of the epoch double buffer (1, 2: the program takes the row as its batch cursor);
+                          // 3: this model's slot of a training group's input, rows X_base.. of the half the launch's batch cursor selects
+    int X_base = 0;       // (X_mode 3)
     const bf16* vstate_b = nullptr;
     const bf16* h0state_b = nullptr;
     bool last_was_tc = false;
@@ -164,7 +166,7 @@ struct RbmTC : RbmSimt<float> {
     void stage_tc(const void* X_host, int64_t first_row, int rows, uint64_t seed, uint32_t tick, uint32_t row0) {
         reserve_tc(rows);
         const bool plain = (cfg.v_kind != BM_UNIT_GAUSSIAN) && (cfg.dropout_keep < 0);
-        X_mode = 0;
+        X_mode = 0; X_base = 0;
         if (staged_half >= 0) {
             // epoch data already converted into a half of Xb by the copy stream (convert_on_copy_stream)
             reserve(rows);
@@ -214,16 +216,16 @@ struct RbmTC : RbmSimt<float> {
         return true;
     }
 
-    // The whole chain (base_rbm.py:421-426, 367-384) -- and, for training, the fused dW
-    // (base_rbm.py:447-448) -- as ONE persistent launch.
-    void run_program(int rows, int k, bool with_dw, uint64_t seed, uint32_t tick, uint32_t row0) {
-        BM_REQUIRE(k >= 1, "n_gibbs_steps must be >= 1");
-        last_plan.clear();
-        const bool resident = X_mode != 0;           // the input is addressed through the launch's batch cursor
-        auto key = std::make_tuple(rows, k, with_dw ? 1 : 0, X_mode);
-        std::unique_ptr<TcProgram>& slot = progs[key];
+    TcProgram& program_for(int rows, int k, bool with_dw) {
+        std::unique_ptr<TcProgram>& slot = progs[std::make_tuple(rows, k, with_dw ? 1 : 0, X_mode)];
         if (!slot) slot.reset(new TcProgram());
-        TcProgram& prog = *slot;
+        return *slot;
+    }
+    // the ops of the chain -- and, with_dw, of the statistics -- over the current input, into prog.ops
+    void build_program(TcProgram& prog, int rows, int k, bool with_dw) {
+        BM_REQUIRE(k >= 1, "n_gibbs_steps must be >= 1");
+        const bool resident = X_mode != 0;           // the input is addressed through the launch's batch cursor
+        const int first_row = resident ? X_base : X_row0;
         const bool sh = cfg.sample_h != 0, sv = cfg.sample_v != 0;
         std::vector<TcGemm>& ops = prog.ops;
         ops.clear();
@@ -232,7 +234,7 @@ struct RbmTC : RbmSimt<float> {
         if (in_program) {
             // rows of the resident dataset beyond this batch only produce output rows >= M, which are masked
             ops.push_back(layer_op(true, mat(X_b, X_rows_total, V, X_ld), resident, h0m_b.p, h0s_b.p, sh, SITE_H0, 0, rows));
-            if (!resident) ops.back().a_row0[0] = X_row0;
+            ops.back().a_row0[0] = first_row;
             h0state_b = sh ? h0s_b.p : h0m_b.p;
             hstate = h0state_b;
             int prev = 0;
@@ -261,7 +263,7 @@ struct RbmTC : RbmSimt<float> {
             const int row_chunks = (rows + 63) / 64;
             auto operand_x = [&](TcGemm& g, int pr, int cols) {
                 g.A[pr] = mat(X_b, X_rows_total, cols, X_ld); g.a_t[pr] = true; g.a_batch[pr] = resident;
-                if (!resident) g.a_k0[pr] = X_row0;
+                g.a_k0[pr] = first_row;
                 g.K[pr] = rows;
             };
             auto operand_v = [&](TcGemm& g, int pr, int cols) {
@@ -360,6 +362,16 @@ struct RbmTC : RbmSimt<float> {
                 ops.push_back(g);
             }
         }
+    }
+
+    // The whole chain (base_rbm.py:421-426, 367-384) -- and, for training, the fused dW
+    // (base_rbm.py:447-448) -- as ONE persistent launch.
+    void run_program(int rows, int k, bool with_dw, uint64_t seed, uint32_t tick, uint32_t row0) {
+        last_plan.clear();
+        const bool resident = X_mode != 0;
+        TcProgram& prog = program_for(rows, k, with_dw);
+        build_program(prog, rows, k, with_dw);
+        std::vector<TcGemm>& ops = prog.ops;
         if ((int)ops.size() <= TC_PROGRAM_OPS) {
             if (!ops.empty()) launch_tc_program(ctx, prog, make_rng(seed, 0, 0, tick, row0), resident ? X_row0 : 0, &last_plan);
         } else {
@@ -471,10 +483,7 @@ struct RbmTC : RbmSimt<float> {
             std::swap(q.p, q_alt.p);
             return;
         }
-        CdTail t{};
-        t.V = V; t.H = H;
-        t.part = partials.p; t.stride = gstride(); t.splits = dw_splits; t.srow = VP();
-        t.vpart = vparts.p; t.vstride = vstride(); t.vsplits = v_splits;
+        CdTail t = tail(rows, lr, mom);
         if (ctx->nranks > 1) {
             // with peers: sum this rank's slices, one all-reduce over [G' | sum(X - v_k)], then the same update on every rank
             tstats.ensure(gstride() + vstride());
@@ -483,15 +492,49 @@ struct RbmTC : RbmSimt<float> {
             allreduce_sum(ctx, tstats.p, gstride() + vstride(), false);
             t.part = tstats.p; t.splits = 1; t.vpart = tstats.p + gstride(); t.vsplits = 1;
         }
+        launch_cd_tail(ctx, t);
+        std::swap(q.p, q_alt.p);               // (same size; "q_means" names the current one)
+    }
+
+    // the update of the step whose program has just been built (its statistics are the split-K slices of this rank)
+    CdTail tail(int rows, double lr, double mom) const {
+        CdTail t{};
+        t.V = V; t.H = H;
+        t.part = partials.p; t.stride = gstride(); t.splits = dw_splits; t.srow = VP();
+        t.vpart = vparts.p; t.vstride = vstride(); t.vsplits = v_splits;
         t.n_div = (float)((double)rows * ctx->nranks);
         t.lr = (float)lr; t.mom = (float)mom; t.l2 = (float)cfg.l2;
         t.damp = (float)cfg.sparsity_damping; t.cost = (float)cfg.sparsity_cost; t.target = (float)cfg.sparsity_target;
         t.W = W.p; t.dW = dW.p; t.vb = vb.p; t.hb = hb.p; t.dvb = dvb.p; t.dhb = dhb.p;
         t.q_old = q.p; t.q_new = q_alt.p; t.pen = pen.p;
         t.Wb = Wb.p; t.ldwb = ldw;
-        launch_cd_tail(ctx, t);
-        std::swap(q.p, q_alt.p);               // (same size; "q_means" names the current one)
+        return t;
     }
+
+    // ---- training groups (bm_rbm_group.cu) ----
+    TcGroupMember* tc_group_member() override { return this; }
+    TcProgram& group_step(const bf16* X, int ld, int rows_total, int base, int cursor, const float* Xf, int rows, int k) override {
+        reserve_tc(rows);
+        reserve(rows);
+        X_b = X; X_ld = ld; X_rows_total = rows_total; X_base = base; X_row0 = cursor + base; X_mode = 3;
+        Xcur = Xf;
+        last_rows = rows;
+        last_plan.clear();
+        TcProgram& prog = program_for(rows, k, true);
+        build_program(prog, rows, k, true);
+        last_was_tc = true;
+        return prog;
+    }
+    CdTail group_tail(int rows, double lr, double mom) const override { return tail(rows, lr, mom); }
+    void group_step_done() override { std::swap(q.p, q_alt.p); }
+    std::vector<bm_tc_op_plan>& group_plan() override { return last_plan; }
+    void group_metrics(uint32_t mask, int rows, uint64_t seed, uint32_t tick, double* dst) override {
+        double unused[4];
+        defer_dst = dst;
+        try { run_metrics(mask, rows, seed, tick, 0, unused); } catch (...) { defer_dst = nullptr; throw; }
+        defer_dst = nullptr;
+    }
+    void group_finish_metrics(const double* h, uint32_t mask, double* out) const override { finish_metrics(h, mask, out); }
 
     void transform(const void* X_host, int rows, int k, uint64_t seed, uint32_t tick, void* H_out) override {
         if (!tc_kinds) { last_was_tc = false; RbmSimt<float>::transform(X_host, rows, k, seed, tick, H_out); return; }

@@ -924,7 +924,7 @@ tc_program_kernel(const __grid_constant__ TcLaunch L) {
             c.p.out_f32 = ph->out_f32; c.p.ld_f32 = ph->ld_f32; c.p.split_stride = ph->split_stride;
             c.p.ais_a = ph->ais_a; c.p.ais_b = ph->ais_b; c.p.ais_next = ph->ais_next; c.p.ais_lin = ph->ais_lin; c.p.ais_logw = ph->ais_logw;
             c.p.ais_ct = ph->ais_b - ph->ais_a; c.p.ais_cd = ph->ais_next - 0.5f * (ph->ais_a + ph->ais_b);
-            c.rng.k0 = L.k0; c.rng.k1 = L.k1; c.rng.tick = L.tick + ph->tick_off; c.rng.row0 = L.row0; c.rng.c2 = ph->rng_c2;
+            c.rng.k0 = ph->k0; c.rng.k1 = ph->k1; c.rng.tick = L.tick + ph->tick_off; c.rng.row0 = L.row0; c.rng.c2 = ph->rng_c2;
             c.m0 = (u.m_group * CL + crank) * BM + c.r0;
             c.n_blk = u.n_blk; c.split = u.split;
             switch (ph->mode) {
@@ -1094,6 +1094,7 @@ static void fill_phase(Ctx* ctx, const TcGemm& g, int cluster, TcPhase& ph) {
     p.acc_scale = g.acc_scale; p.bias_scale = g.bias_scale;
     p.bias = g.bias; p.sigma = g.sigma; p.noise_sigma = g.noise_sigma;
     p.act = g.act; p.sample = g.sample; p.mode = epilogue_mode(g);
+    p.k0 = g.rng.k0; p.k1 = g.rng.k1;
     p.rng_c2 = g.rng.c2;
     p.ais_kind = g.ais_kind; p.ais_a = g.ais_a; p.ais_b = g.ais_b; p.ais_next = g.ais_next; p.ais_lin = g.ais_lin;
     p.ais_logw = g.ais_logw; p.tick_off = g.tick_off;
@@ -1253,6 +1254,7 @@ void launch_tc_program(Ctx* ctx, TcProgram& prog, RngKey rng, int batch_row, std
     double flops = 0.0;
     for (int i = 0; i < n; ++i) {
         fill_phase(ctx, prog.ops[i], cluster, ph[i]);
+        if (!prog.op_keys) { ph[i].l.k0 = rng.k0; ph[i].l.k1 = rng.k1; }
         ph[i].l.n_units = ph[i].l.m_groups * ph[i].l.n_tiles * ph[i].l.splits;
         unit += ph[i].l.n_units;
         ctr_off[i] = n_ctr;
@@ -1273,10 +1275,16 @@ void launch_tc_program(Ctx* ctx, TcProgram& prog, RngKey rng, int batch_row, std
     {
         const int total = ctx->sm_count / cluster;
         int P = 0;
-        for (int i = 0; i < n; ++i) if (prog.ops[i].lane == LANE_CHAIN) P = std::max(P, ph[i].l.n_units);
+        for (int i = 0; i < n; ++i) if (prog.ops[i].lane == LANE_CHAIN && prog.ops[i].pair_count == 0) P = std::max(P, ph[i].l.n_units);
         if (P > total || P == 0) P = total;
         for (int i = 0; i < n; ++i) {
-            int lane = prog.ops[i].lane;
+            const TcGemm& g = prog.ops[i];
+            if (g.pair_count > 0) {
+                BM_REQUIRE(g.pair_begin >= 0 && g.pair_begin + g.pair_count <= total, "CTA pair range outside the grid");
+                ph[i].l.pair_begin = g.pair_begin; ph[i].l.pair_count = g.pair_count;
+                continue;
+            }
+            int lane = g.lane;
             if (lane == LANE_SPARE && total - P < 1) lane = LANE_ALL;
             ph[i].l.pair_begin = lane == LANE_SPARE ? P : 0;
             ph[i].l.pair_count = lane == LANE_CHAIN ? P : (lane == LANE_SPARE ? total - P : total);

@@ -42,7 +42,7 @@ struct TcGemm {
     const float* noise_sigma = nullptr;
     int act = ACT_LINEAR;
     int sample = SMP_NONE;
-    RngKey rng{};                     // single launches: full key; programs: only c2 (site | t << 8) is used
+    RngKey rng{};                     // single launches: full key; programs: c2 (site | t << 8), and k0 / k1 with TcProgram::op_keys
     __nv_bfloat16* out_mean_bf = nullptr;  int ld_mean_bf = 0;
     __nv_bfloat16* out_state_bf = nullptr; int ld_state_bf = 0;
     float* out_f32 = nullptr;              int ld_f32 = 0;     // fp32 means (or raw accumulators)
@@ -57,6 +57,7 @@ struct TcGemm {
     //   LANE_SPARE: the pairs the chain ops never use (falls back to LANE_ALL when there are none)
     //   LANE_ALL  : every pair
     int lane = 0;
+    int pair_begin = 0, pair_count = 0;   // pair_count > 0: run on pairs [pair_begin, + pair_count) whatever the lane (training groups)
     // AIS in the epilogue (TcPhaseLite::ais_kind and friends)
     int ais_kind = 0;
     float ais_a = 0.f, ais_b = 0.f, ais_next = 0.f, ais_lin = 0.f;
@@ -87,9 +88,10 @@ struct TcProgram {
     std::vector<unsigned char> host_image;      // last uploaded descriptor image
     int epoch = 0;                              // launches since the dataflow counters were last zeroed
     int chain_units = -1;                       // largest unit count of the chain ops (planned once by the owner)
+    bool op_keys = false;                       // ops draw with their own rng.k0 / k1 (training groups), not the launch key
     ~TcProgram();
 };
-// seed/tick/row0 of `rng` are shared by all ops; batch_row shifts the ops' a_batch operands.  `plan` (nullable, tests)
+// tick/row0 of `rng` are shared by all ops, and so is its key unless prog.op_keys; batch_row shifts the ops' a_batch operands.  `plan` (nullable, tests)
 // receives one record per op of the launch, appended once the launch was issued (its `launch` field is left 0).
 void launch_tc_program(Ctx* ctx, TcProgram& prog, RngKey rng, int batch_row, std::vector<bm_tc_op_plan>* plan = nullptr);
 
@@ -119,6 +121,8 @@ void launch_weight_update_splitk(Ctx* ctx, const float* partial, size_t stride, 
                                  int V, int H, const float* pen, float l2, float lr, float mom, __nv_bfloat16* Wb, int ldwb);
 
 void launch_cd_tail(Ctx* ctx, const CdTail& t);
+// the updates of n models of one shape in one launch: dev_tails[n] in device memory, `first` a host copy of its first entry
+void launch_cd_tail_group(Ctx* ctx, const CdTail* dev_tails, const CdTail& first, int n);
 // buf[r, col0] = a, buf[r, col0 + 1] = b for r < rows (the two constant columns of a batch buffer)
 void launch_set_column_pair(Ctx* ctx, __nv_bfloat16* buf, int ld, size_t rows, int col0, float a, float b);
 void launch_fill_bf16(Ctx* ctx, __nv_bfloat16* buf, size_t n, float v);

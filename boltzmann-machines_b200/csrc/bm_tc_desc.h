@@ -24,6 +24,8 @@ struct TcPhaseLite {
     const float* sigma;
     const float* noise_sigma;
     int act, sample, mode;
+    uint32_t k0, k1;                 // Philox key of this op's draws (an engine's own programs: the launch key; training groups:
+                                     // each member's seed)
     uint32_t rng_c2;                 // site | t << 8
     __nv_bfloat16* out_mean_bf;  int ld_mean_bf;
     __nv_bfloat16* out_state_bf; int ld_state_bf;
@@ -60,7 +62,8 @@ struct TcLaunch {
     TcPhase inl;                     // single-op launches carry their descriptor in the parameters
     const TcPhase* phases;           // programs: descriptors in global memory
     int n_phases, total_units;
-    uint32_t k0, k1, tick, row0;     // Philox key / call tick / first global row of this shard
+    uint32_t k0, k1, tick, row0;     // Philox key every op of the launch carries unless it has its own (TcPhaseLite::k0) /
+                                     // call tick / first global row of this shard
     int batch_row;
     int stages, stage_bytes;
     unsigned long long* dbg;

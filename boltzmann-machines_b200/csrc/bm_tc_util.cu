@@ -336,13 +336,14 @@ void launch_weight_update_splitk(Ctx* ctx, const float* partial, size_t stride, 
 
 
 // ---- one launch for the whole update of a CD step (see CdTail in bm_tc.h) -----------------------------------------------
+// block `blk` of the update of one model: blocks [0, w_blocks) update W, the rest the biases
 template <int VEC>
-__global__ void __launch_bounds__(256) cd_tail_kernel(const CdTail t, unsigned w_blocks) {
+__device__ __forceinline__ void cd_tail_block(const CdTail& t, unsigned w_blocks, unsigned blk) {
     const int V = t.V, H = t.H;
-    if (blockIdx.x < w_blocks) {
+    if (blk < w_blocks) {
         // ---- weights: VEC consecutive hidden units of one visible unit per thread ----
         const size_t n = (size_t)V * H;
-        const size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * VEC;
+        const size_t i = ((size_t)blk * blockDim.x + threadIdx.x) * VEC;
         if (i >= n) return;
         const int h = (int)(i % (size_t)H);
         const size_t v = i / (size_t)H;
@@ -392,7 +393,7 @@ __global__ void __launch_bounds__(256) cd_tail_kernel(const CdTail t, unsigned w
         return;
     }
     // ---- biases, sparsity statistics ----
-    const int i = (int)(blockIdx.x - w_blocks) * blockDim.x + threadIdx.x;
+    const int i = (int)(blk - w_blocks) * blockDim.x + threadIdx.x;
     if (i < H) {
         float ds = 0.f, qs = 0.f;
         for (int s = 0; s < t.splits; ++s) {
@@ -416,14 +417,37 @@ __global__ void __launch_bounds__(256) cd_tail_kernel(const CdTail t, unsigned w
         t.vb[i] += d;
     }
 }
-void launch_cd_tail(Ctx* ctx, const CdTail& t) {
-    const bool vec = t.H % 4 == 0 && t.ldwb % 4 == 0 && (t.stride & 3) == 0 && (reinterpret_cast<uintptr_t>(t.part) & 15) == 0;
+template <int VEC>
+__global__ void __launch_bounds__(256) cd_tail_kernel(const CdTail t, unsigned w_blocks) { cd_tail_block<VEC>(t, w_blocks, blockIdx.x); }
+// training groups: model m takes blocks [m * per_model, (m + 1) * per_model)
+template <int VEC>
+__global__ void __launch_bounds__(256) cd_tail_group_kernel(const CdTail* __restrict__ tails, unsigned per_model, unsigned w_blocks) {
+    cd_tail_block<VEC>(tails[blockIdx.x / per_model], w_blocks, blockIdx.x % per_model);
+}
+static bool cd_tail_vec(const CdTail& t) {
+    return t.H % 4 == 0 && t.ldwb % 4 == 0 && (t.stride & 3) == 0 && (reinterpret_cast<uintptr_t>(t.part) & 15) == 0;
+}
+static void cd_tail_blocks(const CdTail& t, bool vec, unsigned* w_blocks, unsigned* b_blocks) {
     const size_t items = ((size_t)t.V * t.H) / (vec ? 4 : 1);
-    const unsigned w_blocks = (unsigned)((items + 255) / 256);
+    *w_blocks = (unsigned)((items + 255) / 256);
     const int nb = t.V > t.H ? t.V : t.H;
-    const unsigned b_blocks = (unsigned)((nb + 255) / 256);
+    *b_blocks = (unsigned)((nb + 255) / 256);
+}
+void launch_cd_tail(Ctx* ctx, const CdTail& t) {
+    const bool vec = cd_tail_vec(t);
+    unsigned w_blocks, b_blocks;
+    cd_tail_blocks(t, vec, &w_blocks, &b_blocks);
     if (vec) cd_tail_kernel<4><<<w_blocks + b_blocks, 256, 0, ctx->stream>>>(t, w_blocks);
     else cd_tail_kernel<1><<<w_blocks + b_blocks, 256, 0, ctx->stream>>>(t, w_blocks);
+    count_launch(ctx);
+}
+void launch_cd_tail_group(Ctx* ctx, const CdTail* dev_tails, const CdTail& first, int n) {
+    const bool vec = cd_tail_vec(first);
+    unsigned w_blocks, b_blocks;
+    cd_tail_blocks(first, vec, &w_blocks, &b_blocks);
+    const unsigned per = w_blocks + b_blocks;
+    if (vec) cd_tail_group_kernel<4><<<per * (unsigned)n, 256, 0, ctx->stream>>>(dev_tails, per, w_blocks);
+    else cd_tail_group_kernel<1><<<per * (unsigned)n, 256, 0, ctx->stream>>>(dev_tails, per, w_blocks);
     count_launch(ctx);
 }
 

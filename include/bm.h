@@ -151,6 +151,36 @@ int  bm_rbm_metrics(bm_rbm* rbm, const void* X, int32_t rows, int32_t n_gibbs_st
  * in BF16 compute mode (widened), cfg.dtype otherwise. */
 int  bm_rbm_get_activation(bm_rbm* rbm, const char* name, void* host, size_t bytes);
 
+/* ---- training groups: many RBMs of one shape trained side by side (no counterpart in the reference) ----------------
+ * A group drives the training steps of n ordinary bm_rbm handles.  Step i of a group epoch runs, for every member m, exactly
+ * what bm_rbm_train_epoch step i of that member runs: the same ops, tile widths, splits and K orders, the same draws from
+ * the member's own seed and tick, the same update -- so every variable and metric is bit-identical to the member's own epoch.
+ * The members' chains share the program launches of a step (each member on its own CTA pairs; a step whose ops do not fit
+ * one launch is cut between members) and one launch updates all of them.  The members stay ordinary handles: get_param,
+ * set_param, metrics, transform and bm_rbm_debug_tc_plan work on them as before (the plan then shows the grouped launch).
+ * Members must share the context, n_visible, n_hidden, the unit kinds and max_batch (BM_EINVAL naming the field); seeds,
+ * sigma, l2, the sparsity settings, dbm_first / dbm_last and the sampling flags may differ.  BM_EUNSUPPORTED, with the
+ * option named: multinomial layers, the fp32 / fp64 engines (only BM_COMPUTE_BF16 members), dropout and a context with a
+ * communicator. */
+typedef struct bm_rbm_group bm_rbm_group;
+int  bm_rbm_group_create(bm_ctx* ctx, bm_rbm* const* members, int32_t n, bm_rbm_group** out);
+void bm_rbm_group_destroy(bm_rbm_group* group);
+/* One epoch of every member over X[n][n_rows][n_visible] (member m trains on X[m]; cfg.dtype, bytes or bfloat16 bit
+ * patterns as in bm_rbm_train_epoch / _u8 / _bf16).  Per member m: lr[m], momentum[m], seeds[m], tick0[m], metric_mask[m],
+ * metrics_every[m] and iter0[m] mean what they mean for bm_rbm_train_epoch; n_gibbs_steps is shared and at most 43 (a longer
+ * chain needs several launches per member).  out[(m * n_batches + i) * 4 ..] receives member m's metrics of batch i (zeros
+ * on batches that do not report); out may be NULL when every mask is 0.  Uploads are double-buffered on the copy stream:
+ * one host->device copy and one conversion per step for all members. */
+int  bm_rbm_group_train_epoch(bm_rbm_group* group, const void* X, int64_t n_rows, int32_t batch, const double* lr,
+                              const double* momentum, int32_t n_gibbs_steps, const uint64_t* seeds, const uint32_t* tick0,
+                              const uint32_t* metric_mask, const int32_t* metrics_every, const int64_t* iter0, double* out);
+int  bm_rbm_group_train_epoch_u8(bm_rbm_group* group, const uint8_t* X, int64_t n_rows, int32_t batch, const double* lr,
+                                 const double* momentum, int32_t n_gibbs_steps, const uint64_t* seeds, const uint32_t* tick0,
+                                 const uint32_t* metric_mask, const int32_t* metrics_every, const int64_t* iter0, double* out);
+int  bm_rbm_group_train_epoch_bf16(bm_rbm_group* group, const uint16_t* X, int64_t n_rows, int32_t batch, const double* lr,
+                                   const double* momentum, int32_t n_gibbs_steps, const uint64_t* seeds, const uint32_t* tick0,
+                                   const uint32_t* metric_mask, const int32_t* metrics_every, const int64_t* iter0, double* out);
+
 /* ---- DBM -------------------------------------------------------------------------------------
  * Static configuration: what DBM._make_constants/_make_vars bake into the graph (dbm.py:233-383).
  * Per-layer arrays have n_layers entries (hidden layer 0 is adjacent to the visibles). */
