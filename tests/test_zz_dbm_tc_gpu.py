@@ -214,21 +214,35 @@ def test_ais_at_the_benchmark_shape_is_within_one_nat_of_the_float64_oracle():
     eng.close(); simt.close()
 
 
+CFG4_INCREMENT_REL = 0.1
+
+
 def test_cfg4_shape_step_agrees_with_the_fp32_engine():
-    """BASELINE.json configs[3] shape: DBM 784-512-1024, 1024 particles, batch 1024, 25 mean-field updates."""
+    """BASELINE.json configs[3] shape: DBM 784-512-1024, 1024 particles, batch 1024, 25 mean-field updates.  The two engines'
+    increments (W - W0, vb - vb0, ...) agree to CFG4_INCREMENT_REL of their norm: one step moves W by about 1 % of its norm, so
+    the parameters themselves would agree even if the update were skipped (a skipped update gives 1.0 here).  The increments
+    differ by the bf16 rounding of the operands and by the draws it flips; measured on an H100 SXM (700 W): W 0.0054, W_1 0.030,
+    vb 0.0032, hb 0.014, hb_1 0.047.  Every variable of the step is replayed against float64 in
+    tests/test_zz_dbm_tc_replay_gpu.py."""
     base = make_cfg(V=784, Hs=(512, 1024), n_particles=1024, batch_size=1024, max_mf_updates=25, mf_tol=1e-7,
                     max_norm=6.0, sparsity_cost=[0., 0.])
     tc, simt = _native.CudaDBM(base), _native.CudaDBM(dict(base, compute='fp32'))
     assert tc.compute == 'bf16' and simt.compute == 'fp32'
     init(base, (tc, simt), scale=0.02)
+    names = ['W', 'W_1', 'vb', 'hb', 'hb_1']
+    p0 = tc.get_params(names)
     X = batch(base, 1024)
     a = tc.train_step(X, 2e-3, 0.5, 1, 7, 0, metrics=('msre', 'n_mf_updates'))
     b = simt.train_step(X, 2e-3, 0.5, 1, 7, 0, metrics=('msre', 'n_mf_updates'))
     assert a['msre'] == pytest.approx(b['msre'], rel=0.02)
-    ga, gb = tc.get_params(['W', 'W_1', 'vb', 'hb', 'hb_1']), simt.get_params(['W', 'W_1', 'vb', 'hb', 'hb_1'])
-    for k in ga:
-        rel = np.linalg.norm(ga[k] - gb[k]) / max(np.linalg.norm(gb[k]), 1e-12)
-        assert rel < 0.02, (k, rel)
+    ga, gb = tc.get_params(names), simt.get_params(names)
+    rels = {}
+    for k in names:
+        da, db = ga[k].astype(np.float64) - p0[k], gb[k].astype(np.float64) - p0[k]
+        assert np.linalg.norm(db) > 0, k
+        rels[k] = np.linalg.norm(da - db) / np.linalg.norm(db)
+    print('\n[cfg4 increments] relative difference bf16 vs fp32 engine:', {k: round(float(v), 5) for k, v in rels.items()})
+    assert max(rels.values()) < CFG4_INCREMENT_REL, rels
     tc.close(); simt.close()
 
 
