@@ -202,6 +202,7 @@ void bm_ctx_destroy(bm_ctx* h) {
     for (cudaEvent_t e : c->prof_events) cudaEventDestroy(e);
     if (c->l2_scratch) cudaFree(c->l2_scratch);
     if (c->sqdiff_scratch) cudaFree(c->sqdiff_scratch);
+    if (c->reduce_scratch) cudaFree(c->reduce_scratch);
     if (c->colsum_scratch) cudaFree(c->colsum_scratch);
     cudaEventDestroy(c->t0); cudaEventDestroy(c->t1); cudaEventDestroy(c->copy_done);
     cudaStreamDestroy(c->stream); cudaStreamDestroy(c->copy_stream);

@@ -64,6 +64,7 @@ struct Ctx {
     uint64_t prof_launches = 0;
     // scratch of the small reduction kernels: per CONTEXT (two contexts on one device run on different streams)
     double* sqdiff_scratch = nullptr;
+    double* reduce_scratch = nullptr;    // partial sums of sqdiff_mean / sumsq (bm_simt.cu)
     float* colsum_scratch = nullptr;
     size_t colsum_scratch_floats = 0;
     // NCCL (resolved at run time with dlopen; see bm_comm.cu)

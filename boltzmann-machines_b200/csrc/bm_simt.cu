@@ -331,11 +331,10 @@ __global__ void finish_sum_kernel(const double* __restrict__ partial, int n, dou
     if (threadIdx.x == 0) *out = sh[0] / denom;
 }
 static double* g_partials(Ctx* ctx) {
-    // one scratch array of partial sums per context would be cleaner; a process-wide one per
-    // device is enough because every launch is stream-ordered on ctx->stream
-    static double* buf[64] = {nullptr};
-    if (!buf[ctx->device]) BM_CUDA(cudaMalloc(&buf[ctx->device], 1024 * sizeof(double)));
-    return buf[ctx->device];
+    // per context: the partial sums are written and read on ctx->stream, and two contexts on one device run their
+    // reductions on two streams that are not ordered against each other
+    if (!ctx->reduce_scratch) BM_CUDA(cudaMalloc(&ctx->reduce_scratch, 1024 * sizeof(double)));
+    return ctx->reduce_scratch;
 }
 template <typename T>
 void launch_sqdiff_mean(Ctx* ctx, const T* P, int ldp, const T* Q, int ldq, int rows, int cols,

@@ -161,7 +161,13 @@ class OracleRBM(object):
 
     def prepare_input(self, X, seed, tick, row0=0):
         """GaussianRBM pre-division (rbm/rbm.py:101-107) then dropout
-        (base_rbm.py:417-418)."""
+        (base_rbm.py:417-418); in bf16 mode rounded to bf16 like the chain's
+        input operand."""
+        return self._r(self.prepare_input_fp(X, seed, tick, row0))
+
+    def prepare_input_fp(self, X, seed, tick, row0=0):
+        """The prepared batch before any bf16 rounding: what the free energy
+        and the PLL read in every mode."""
         X = np.asarray(X, dtype=self.dt)
         if self.v_kind == 'gaussian':
             X = X / self.sigma[None, :]
@@ -170,7 +176,7 @@ class OracleRBM(object):
             u = P.uniform_at(X.shape[0], X.shape[1], seed, P.SITE_DROPOUT, 0, tick, row0)
             mask = np.floor(np.float32(keep) + u).astype(self.dt)
             X = X / self.dt.type(keep) * mask
-        return self._r(X)
+        return X
 
     def chain(self, X, k, seed, tick, row0=0):
         """base_rbm.py:421-426 + :367-384.  X is the prepared batch."""
@@ -198,8 +204,11 @@ class OracleRBM(object):
         return h0_means, v_states, v_means, h_states, h_means
 
     # -- free energies (rbm/rbm.py:17-22, 50-60, 109-116) --------------------
+    # In bf16 mode too they read the fp32 W and the unrounded prepared batch: the
+    # engine evaluates them on its CUDA-core kernels in fp32, as the reference's
+    # graph does (only the chain and MSRE see bf16 operands).
     def free_energy(self, v, seed=0, tick=0, fe_idx=0):
-        W = self._Wc()
+        W = self.p['W']
         if self.h_kind == 'multinomial':
             K, M = self.H, float(self.cfg.get('h_n_samples', 100))
             from math import lgamma
@@ -228,16 +237,19 @@ class OracleRBM(object):
         d = self.free_energy(Xc, seed, tick, 0) - self.free_energy(X, seed, tick, 1)
         return float(self.V * -np.logaddexp(0.0, -d))
 
-    def _metrics(self, names, X, v_means, seed, tick, row0):
+    def _metrics(self, names, X, v_means, seed, tick, row0, X_fp=None):
+        """X: the chain's input (MSRE); X_fp: the same batch unrounded (free
+        energy, PLL), X itself when not given."""
+        X_fp = X if X_fp is None else X_fp
         out = {}
         if 'l2_loss' in names:   # base_rbm.py:482-484
             out['l2_loss'] = float(self.cfg.get('l2', 0.) * 0.5 * np.sum(np.square(self.p['W'], dtype=np.float64)))
         if 'msre' in names:      # :486-488
             out['msre'] = float(np.mean(np.square(X - v_means), dtype=np.float64))
         if 'pll' in names:
-            out['pll'] = self.pll(X, seed, tick, row0)
+            out['pll'] = self.pll(X_fp, seed, tick, row0)
         if 'free_energy' in names:   # :516
-            out['free_energy'] = self.free_energy(X, seed, tick, 2)
+            out['free_energy'] = self.free_energy(X_fp, seed, tick, 2)
         return out
 
     # -- engine interface ----------------------------------------------------
@@ -252,9 +264,10 @@ class OracleRBM(object):
         c, p, dt = self.cfg, self.p, self.dt
         rank, nranks, allreduce = shard if shard is not None else (0, 1, None)
         row0 = rank * np.asarray(X).shape[0]
-        X = self.prepare_input(X, seed, tick, row0)
+        X_fp = self.prepare_input_fp(X, seed, tick, row0)
+        X = self._r(X_fp)
         h0_means, v_states, v_means, _, h_means = self.chain(X, k, seed, tick, row0)
-        out = self._metrics(metrics, X, v_means, seed, tick, row0) if metrics else None
+        out = self._metrics(metrics, X, v_means, seed, tick, row0, X_fp) if metrics else None
         self.apply_update(X, h0_means, v_states, h_means, lr, momentum, nranks, allreduce)
         return out
 
@@ -292,11 +305,12 @@ class OracleRBM(object):
 
     def metrics(self, X, k, seed, tick, names):
         """base_rbm.py:573-590 / :592-621 (no parameter update)."""
-        Xp = self.prepare_input(X, seed, tick)
+        X_fp = self.prepare_input_fp(X, seed, tick)
+        Xp = self._r(X_fp)
         v_means = None
         if 'msre' in names:
             v_means = self.chain(Xp, k, seed, tick)[2]
-        return self._metrics(names, Xp, v_means, seed, tick, 0)
+        return self._metrics(names, Xp, v_means, seed, tick, 0, X_fp)
 
     def close(self):
         pass

@@ -12,6 +12,7 @@ import pytest
 from boltzmann_machines import _native
 from oracle.rbm import OracleRBM
 from oracle.dbm import OracleDBM
+from test_zz_rbm_metrics_gpu import Statement, check_metrics
 
 pytestmark = pytest.mark.gpu
 
@@ -60,9 +61,15 @@ def test_rbm_two_steps_on_random_shapes(i, compute):
         assert np.all(np.isfinite(g[name])), name
         np.testing.assert_allclose(g[name], w[name], atol=tol, err_msg='{0} {1}'.format(name, cfg))
     m_g = eng.metrics(X[0], k, 7, 9, ('msre', 'pll', 'free_energy') if cfg['h_kind'] != 'multinomial' else ('msre',))
-    m_w = ora.metrics(X[0], k, 7, 9, tuple(m_g))
-    for name in m_g:
-        assert m_g[name] == pytest.approx(m_w[name], rel=2e-2, abs=2e-2), (name, cfg)
+    # MSRE follows the chain, whose draws may part from the oracle's at rounding-level ties
+    m_w = ora.metrics(X[0], k, 7, 9, ('msre',))
+    assert m_g['msre'] == pytest.approx(m_w['msre'], rel=2e-2, abs=2e-2), ('msre', cfg)
+    # free energy and PLL do not depend on the draws: the float64 statement at the engine's own parameters and prepared batch
+    # (dropout included), within the bound of the engine's fp32 arithmetic (tests/test_zz_rbm_metrics_gpu.py)
+    fe = {n: m_g[n] for n in ('pll', 'free_energy') if n in m_g}
+    if fe:
+        Xp = OracleRBM(dict(cfg, compute='fp32')).prepare_input_fp(X[0], 7, 9)
+        check_metrics(fe, Statement(cfg, g).metrics(tuple(fe), Xp, 7, 9), str(cfg))
     eng.close()
 
 
