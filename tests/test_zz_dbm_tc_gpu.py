@@ -194,7 +194,8 @@ def test_ais_at_the_benchmark_shape_is_within_one_nat_of_the_float64_oracle():
     """north_star's gate at BASELINE.json configs[3]'s own shape: DBM 784-512-1024, 256 runs x 1000 betas -- the tensor-core
     ladder (bf16 operands, epilogue-fused) against the float64 oracle on identical weights, and against the fp32 CUDA-core
     engine (same chains up to rounding).  The oracle's 256 log-weights are a committed fixture (minutes of numpy:
-    tests/golden/make_ais_benchmark_oracle.py; tests/test_oracle_fixtures.py re-derives some of its chains on the CPU)."""
+    tests/golden/make_ais_benchmark_oracle.py; tests/test_oracle_fixtures.py re-derives some of its chains on the CPU).
+    The per-run check of the same ladder is tests/test_zz_dbm_ais_replay_gpu.py."""
     import json
     fx = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'ais_benchmark_shape_oracle.json')))
     sh = fx['shape']
