@@ -30,7 +30,7 @@ EXPORTS = (
     'bm_rbm_get_activation', 'bm_debug_tc_gemm', 'bm_debug_tc_op', 'bm_rbm_debug_tc_plan',
     'bm_dbm_create', 'bm_dbm_destroy', 'bm_dbm_set_param', 'bm_dbm_get_param', 'bm_dbm_init_particles',
     'bm_dbm_train_step', 'bm_dbm_val_metrics', 'bm_dbm_transform', 'bm_dbm_reconstruct', 'bm_dbm_log_proba',
-    'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows', 'bm_debug_dbm_multinomial_rows',
+    'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows', 'bm_dbm_pt_counts', 'bm_debug_dbm_multinomial_rows',
     'bm_crbm_create', 'bm_crbm_destroy', 'bm_crbm_set_param', 'bm_crbm_get_param', 'bm_crbm_init_weights',
     'bm_crbm_train_step', 'bm_crbm_predict_proba', 'bm_crbm_transform',
     'bm_rbm_group_create', 'bm_rbm_group_destroy', 'bm_rbm_group_train_epoch', 'bm_rbm_group_train_epoch_u8',
@@ -68,6 +68,8 @@ class DbmCfg(C.Structure):
         ('sparsity_target', C.POINTER(C.c_double)),
         ('sparsity_cost', C.POINTER(C.c_double)),
         ('sigma', C.POINTER(C.c_double)),
+        ('n_temps', C.c_int32),
+        ('betas', C.POINTER(C.c_double)),
     ]
 
 
@@ -159,6 +161,7 @@ def load_library(path=None):
         'bm_dbm_log_proba': [vp, vp, i32, vp], 'bm_dbm_sample_v': [vp, i32, u64, u32, vp],
         'bm_dbm_ais': [vp, i32, i32, i32, u64, vp],
         'bm_dbm_ais_rows': [vp, i32, i32, i32, u64, u32, vp],
+        'bm_dbm_pt_counts': [vp, vp, vp],
         'bm_debug_dbm_multinomial_rows': [vp, vp, i32, i32, dbl, i32, u64, u32, u32, u32, vp, vp, vp, vp],
         'bm_crbm_create': [vp, C.POINTER(CrbmCfg), C.POINTER(vp)],
         'bm_crbm_set_param': [vp, C.c_char_p, vp, sz], 'bm_crbm_get_param': [vp, C.c_char_p, vp, sz],
@@ -781,8 +784,22 @@ class CudaDBM(object):
         if cfg.get('sigma', None) is not None:
             self._sigma = np.ascontiguousarray(np.broadcast_to(np.asarray(cfg['sigma'], dtype=np.float64), (self.V,)))
             c.sigma = self._sigma.ctypes.data_as(C.POINTER(C.c_double))
+        # parallel tempering: the ladder of inverse temperatures (None: off).  The engine validates it; its refusals of the
+        # option (messages starting 'parallel tempering') surface as NotImplementedError (BM_EUNSUPPORTED) or ValueError
+        # (BM_EINVAL), every other failure of bm_dbm_create as RuntimeError, as without tempering
+        betas = cfg.get('pt_betas', None)
+        self.pt_betas = None if betas is None else np.ascontiguousarray(np.asarray(betas, dtype=np.float64).ravel())
+        self.T = 1 if self.pt_betas is None else len(self.pt_betas)
+        if self.pt_betas is not None:
+            c.n_temps = len(self.pt_betas)
+            c.betas = self.pt_betas.ctypes.data_as(C.POINTER(C.c_double))
         h = C.c_void_p()
-        check(self._lib.bm_dbm_create(self.ctx.handle, C.byref(c), C.byref(h)))
+        rc = self._lib.bm_dbm_create(self.ctx.handle, C.byref(c), C.byref(h))
+        if rc in (-1, -5):
+            err = self._lib.bm_last_error().decode('utf-8', 'replace')
+            if err.startswith('parallel tempering'):
+                raise (NotImplementedError if rc == -5 else ValueError)('libbm: ' + err)
+        check(rc)
         self.handle = h
         self._shapes = {'vb': (self.V,), 'dvb': (self.V,), 'v': (self.M, self.V)}
         sizes = [self.V] + self.Hs
@@ -791,7 +808,17 @@ class CudaDBM(object):
             self._shapes.update({'W' + s: (sizes[i], sizes[i + 1]), 'dW' + s: (sizes[i], sizes[i + 1]),
                                  'hb' + s: (self.Hs[i],), 'dhb' + s: (self.Hs[i],), 'mu' + s: (self.B, self.Hs[i]),
                                  'q_means' + s: (self.Hs[i],), 'mu_means' + s: (self.Hs[i],), 'h' + s: (self.M, self.Hs[i])})
+        if self.T > 1:                     # the tempered slots 1..T-1 of the particles
+            self._shapes['v_pt'] = (self.T - 1, self.M, self.V)
+            for i in range(self.L):
+                self._shapes['h_pt' + _sfx(i)] = (self.T - 1, self.M, self.Hs[i])
         self._out2 = (C.c_double * 2)()
+
+    def pt_counts(self):
+        """(accepted, proposed): int64 arrays of T-1 swap counts between slots m and m+1 since the engine was created."""
+        acc, prop = np.zeros(self.T - 1, dtype=np.int64), np.zeros(self.T - 1, dtype=np.int64)
+        check(self._lib.bm_dbm_pt_counts(self.handle, acc.ctypes.data, prop.ctypes.data))
+        return acc, prop
 
     def set_params(self, d):
         for k, v in d.items():

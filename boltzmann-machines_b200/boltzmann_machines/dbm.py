@@ -45,6 +45,12 @@ class DBM(EnergyBasedModel):
     sparsity_target, sparsity_cost : scalar or per-layer; sparsity_damping
     train_metrics_every_iter, val_metrics_every_epoch, verbose, save_after_each_epoch
     display_filters, display_particles, v_shape : accepted for compatibility
+    pt_betas : None (default), or a ladder of inverse temperatures 1 = b_0 > b_1 > ... > b_{T-1} >= 0 for parallel
+        tempering of the persistent chains (not in the reference; Desjardins et al., AISTATS 2010): slot m holds
+        ``n_particles`` chains swept at b_m, and every particle update ends with one round of swaps between neighbouring
+        slots.  The gradient, ``sample_v`` and the particles ``v`` / ``h...`` are slot 0's.  Needs the tensor-core engine
+        (float32, Bernoulli units) and sampled states in every layer; ``pt_swap_rates_`` holds the last epoch's
+        acceptance rate of each pair (m, m+1) (None for a pair the epoch did not propose).
     """
     _MUTABLE_PREFIXES = ('mu', 'v', 'h')
 
@@ -58,7 +64,7 @@ class DBM(EnergyBasedModel):
                  train_metrics_every_iter=10, val_metrics_every_epoch=1,
                  verbose=False, save_after_each_epoch=True,
                  display_filters=0, display_particles=0, v_shape=(28, 28),
-                 model_path='dbm_model/', *args, **kwargs):
+                 model_path='dbm_model/', pt_betas=None, *args, **kwargs):
         super(DBM, self).__init__(model_path=model_path, *args, **kwargs)
         self.n_layers_ = len(rbms) if rbms is not None else None
         self.n_visible_ = None
@@ -107,9 +113,30 @@ class DBM(EnergyBasedModel):
         if len(self.v_shape) == 2:
             self.v_shape = self.v_shape + (1,)
 
+        self.pt_betas = None if pt_betas is None else [float(b) for b in np.asarray(pt_betas, dtype=np.float64).ravel()]
+        self._check_pt()
+        self.pt_swap_rates_ = None
+
         self.epoch_ = 0
         self.iter_ = 0
         self.n_samples_generated_ = 0
+
+    def _check_pt(self):
+        """The refusals of the engine (include/bm.h, bm_dbm_cfg.n_temps) as far as the constructor can tell."""
+        if self.pt_betas is None:
+            return
+        b = self.pt_betas
+        if not b or b[0] != 1.0 or not all(np.isfinite(x) for x in b) or any(y >= x for x, y in zip(b, b[1:])) or b[-1] < 0:
+            raise ValueError('pt_betas must decrease strictly from 1.0 and stay >= 0, got {0}'.format(b))
+        if not self.sample_v_states or not all(self.sample_h_states or []):
+            raise ValueError('parallel tempering needs sampled states in every layer (sample_v_states, sample_h_states)')
+        if np.dtype(self.dtype) != np.float32:
+            raise NotImplementedError('parallel tempering runs on the tensor-core engine: float32 models only')
+        if self.layers_ is not None:
+            if self.layers_['v']['kind'] != 'bernoulli':
+                raise NotImplementedError('parallel tempering is not supported with gaussian visibles')
+            if any(h['kind'] != 'bernoulli' for h in self.layers_['h']):
+                raise NotImplementedError('parallel tempering is not supported with multinomial hidden layers')
 
     # ---- composition from pre-trained RBMs (dbm.py:207-231, 266-291) ---------------------
     def load_rbms(self, rbms):
@@ -157,18 +184,19 @@ class DBM(EnergyBasedModel):
     def _scopes(self):
         L = self.n_layers_ or 0
         per = lambda stem: tuple(stem + _sfx(i) for i in range(L))
+        tempered = ('v_pt',) + per('h_pt') if self.pt_betas is not None and len(self.pt_betas) > 1 else ()
         return {
             'weights': ('vb',) + per('W') + per('hb'),
             'grads_accumulators': ('dvb',) + per('dW') + per('dhb'),
             'variational_params': per('mu'),
             'hidden_means_accumulators': per('q_means') + per('mu_means'),
-            'negative_particles': ('v',) + per('h'),
+            'negative_particles': ('v',) + per('h') + tempered,
         }
 
     def _tf_name(self, scope, name):
         # the hidden particles are created inside `tf.name_scope('h_particle')` (dbm.py:371-383): TF names them
         # negative_particles/h_particle/h, negative_particles/h_particle_1/h, ...
-        if scope == 'negative_particles' and name.startswith('h'):
+        if scope == 'negative_particles' and name.startswith('h') and not name.startswith('h_pt'):
             i = name[2:]
             return 'h_particle{0}/h'.format('_' + i if i else '')
         return name
@@ -189,6 +217,8 @@ class DBM(EnergyBasedModel):
             sparsity_cost=[float(x) for x in self.sparsity_cost],
             sparsity_damping=float(self.sparsity_damping),
         )
+        if self.pt_betas is not None:
+            cfg['pt_betas'] = list(self.pt_betas)
         if 'sigma' in lay['v']:
             cfg['sigma'] = np.broadcast_to(np.asarray(lay['v']['sigma'], dtype=np.float64), (self.n_visible_,)).copy()
         return cfg
@@ -236,6 +266,9 @@ class DBM(EnergyBasedModel):
 
     # ---- training ------------------------------------------------------------------------------------
     def _train_epoch(self, X):
+        pt = self.pt_betas is not None and len(self.pt_betas) > 1
+        if pt:
+            acc0, prop0 = self._engine.pt_counts()
         msres, n_mfs = [], []
         for lo, hi in _maybe_bar(batch_bounds(len(X), self.batch_size), self.verbose, leave=False, ncols=64, desc='epoch'):
             self.iter_ += 1
@@ -246,6 +279,13 @@ class DBM(EnergyBasedModel):
                 msres.append(got['msre']); n_mfs.append(got['n_mf_updates'])
                 self._log_scalars('train', self.iter_, {'mean_squared_recon_error': got['msre'],        # dbm.py:636-639
                                                         'n_mf_updates': got['n_mf_updates']})
+        if pt:                             # the epoch's swap acceptance rate of each neighbouring pair (m, m+1)
+            acc1, prop1 = self._engine.pt_counts()
+            dp = (prop1 - prop0).astype(np.float64)
+            # None for a pair not proposed in the epoch (params.json stays standard JSON)
+            self.pt_swap_rates_ = [float(a) / float(p) if p > 0 else None for a, p in zip(acc1 - acc0, dp)]
+            self._log_scalars('train', self.iter_, {'pt_swap_acceptance_{0}'.format(m): r
+                                                    for m, r in enumerate(self.pt_swap_rates_) if r is not None})
         return (float(np.mean(msres)) if msres else None, float(np.mean(n_mfs)) if n_mfs else None)
 
     def _run_val_metrics(self, X_val):

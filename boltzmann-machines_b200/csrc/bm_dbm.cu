@@ -197,7 +197,28 @@ struct DbmBase {
     virtual void sample_v(int k, uint64_t seed, uint32_t tick, void* out) = 0;
     virtual void ais(int n_runs, int n_betas, int k, uint64_t seed, double* out) = 0;
     virtual void ais_rows(int n_runs, int n_betas, int k, uint64_t seed, uint32_t first_run, double* out) = 0;
+    virtual void pt_counts(int64_t*, int64_t*) { throw Error(BM_EINVAL, "this DBM has no tempered chains (bm_dbm_cfg.n_temps)"); }
 };
+
+// Parallel tempering (bm_dbm_cfg.n_temps / betas): what the engines refuse before anything is allocated.  0 / NULL is off.
+static void check_pt_cfg(const Ctx* ctx, const bm_dbm_cfg& f) {
+    if (f.n_temps == 0 && f.betas == nullptr) return;
+    BM_REQUIRE(f.n_temps >= 1 && f.betas != nullptr, "parallel tempering: n_temps >= 1 inverse temperatures are needed in betas");
+    BM_REQUIRE(f.betas[0] == 1.0, "parallel tempering: betas[0] must be 1");
+    for (int m = 1; m < f.n_temps; ++m)
+        BM_REQUIRE(std::isfinite(f.betas[m]) && f.betas[m] < f.betas[m - 1] && f.betas[m] >= 0.0,
+                   "parallel tempering: betas must decrease strictly from 1 and stay >= 0");
+    if (f.dtype != BM_DTYPE_F32 || f.compute != BM_COMPUTE_BF16)
+        throw Error(BM_EUNSUPPORTED, "parallel tempering runs on the tensor-core engine only (float32 models, compute bf16)");
+    if (f.v_kind != BM_UNIT_BERNOULLI)
+        throw Error(BM_EUNSUPPORTED, "parallel tempering is not supported with gaussian visibles (a tempered gaussian needs variance sigma^2 / beta)");
+    for (int i = 0; i < f.n_layers; ++i)
+        if (f.h_kinds[i] != BM_UNIT_BERNOULLI) throw Error(BM_EUNSUPPORTED, "parallel tempering is not supported with multinomial hidden layers");
+    if (ctx->nranks > 1) throw Error(BM_EUNSUPPORTED, "parallel tempering is not supported on a context with a communicator");
+    BM_REQUIRE(f.sample_v != 0, "parallel tempering needs sampled visible states (sample_v): the swap compares energies of states");
+    for (int i = 0; i < f.n_layers; ++i)
+        BM_REQUIRE(f.sample_h[i] != 0, "parallel tempering needs sampled hidden states (sample_h of every layer): the swap compares energies of states");
+}
 
 template <typename T>
 struct Dbm : DbmBase {
@@ -692,6 +713,8 @@ int bm_dbm_create(bm_ctx* hctx, const bm_dbm_cfg* cfg, bm_dbm** out) {
     BM_REQUIRE(cfg->n_hiddens && cfg->h_kinds && cfg->sample_h && cfg->sparsity_target && cfg->sparsity_cost, "missing per-layer arrays");
     BM_REQUIRE(cfg->n_particles > 0 && cfg->batch_size > 0, "n_particles and batch_size must be positive");
     BM_REQUIRE(cfg->v_kind != BM_UNIT_GAUSSIAN || cfg->sigma, "gaussian visible layer needs sigma");
+    check_pt_cfg(ctx, *cfg);
+    if (cfg->n_temps >= 1 && !DbmTC::supports(*cfg)) throw Error(BM_EUNSUPPORTED, "parallel tempering: the model does not run on the tensor-core engine");
     BM_CUDA(cudaSetDevice(ctx->device));
     // BM_COMPUTE_BF16 (the Python mirror's default): float32 models with Bernoulli hidden layers run their GEMMs on the tensor
     // cores; every other combination keeps the storage-precision CUDA-core engine (as bm_rbm_create does for unit kinds the
@@ -746,6 +769,9 @@ int bm_dbm_ais(bm_dbm* h, int32_t n_runs, int32_t n_betas, int32_t k, uint64_t s
 }
 int bm_dbm_ais_rows(bm_dbm* h, int32_t n_runs, int32_t n_betas, int32_t k, uint64_t seed, uint32_t first_run, double* logZ) {
     BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(logZ, "null argument"); DBM(h)->ais_rows(n_runs, n_betas, k, seed, first_run, logZ); BM_API_END
+}
+int bm_dbm_pt_counts(bm_dbm* h, int64_t* accepted, int64_t* proposed) {
+    BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(accepted && proposed, "null argument"); DBM(h)->pt_counts(accepted, proposed); BM_API_END
 }
 
 int bm_debug_dbm_multinomial_rows(bm_ctx* hctx, const float* pre, int32_t rows, int32_t cols, double n_samples, int32_t n_draws,

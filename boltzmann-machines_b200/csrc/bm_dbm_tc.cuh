@@ -269,6 +269,66 @@ __global__ void ais_fused_step_kernel(double* __restrict__ logw, float a, float 
     if (lane == 0) logw[r] += acc;
 }
 
+// ---- parallel tempering: the swap round ------------------------------------------------------------
+// Slot m of the ladder holds rows [m M, (m+1) M) of every bf16 particle buffer x[0] = v, x[1 + i] = h_i.  P[i] [T M, H_i] holds
+// the raw products h_{i-1} W_i + c_i of the same states (one fp32 tensor-core op per layer), so that
+//   -E(x) = v.b + sum_i h_i . (h_{i-1} W_i + c_i).
+struct PtSwapArgs {
+    int L, T, M, V;
+    int H[8];
+    int ld[9];
+    bf16_t* x[9];
+    const float* P[8];
+    const float* vb;
+    const double* betas;            // [T] device
+    int parity;                     // pairs (m, m+1) with m % 2 == parity are proposed
+    RngKey rng;                     // seed, tick, row0 of the swap draws (site and t are set per pair)
+    unsigned long long* accepted;   // [T - 1], cumulative
+};
+// One 256-thread block per particle p: the T energies of its slots (one warp per slot; per lane a strided sum in double, then
+// the xor tree), the decision of every proposed pair (u from Philox (SITE_DBM_PT, t = m) at column 0 of row row0 + p; accept
+// when log u < (beta_m - beta_{m+1}) (E_m - E_{m+1})), then the exchange of the accepted pairs' rows in every particle buffer.
+// The proposed pairs are disjoint, so the exchanges never touch one row twice.  Dynamic shared memory: T doubles + T ints.
+__global__ void __launch_bounds__(256) dbm_pt_swap_kernel(PtSwapArgs a) {
+    extern __shared__ double pt_smem[];
+    double* E = pt_smem;
+    int* acc = reinterpret_cast<int*>(pt_smem + a.T);
+    const int p = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int m = warp; m < a.T; m += 8) {
+        const size_t row = (size_t)m * a.M + p;
+        double s = 0.0;
+        for (int j = lane; j < a.V; j += 32) s += (double)__bfloat162float(a.x[0][row * a.ld[0] + j]) * (double)a.vb[j];
+        for (int i = 0; i < a.L; ++i)
+            for (int j = lane; j < a.H[i]; j += 32)
+                s += (double)__bfloat162float(a.x[i + 1][row * a.ld[i + 1] + j]) * (double)a.P[i][row * a.H[i] + j];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        if (lane == 0) E[m] = -s;
+    }
+    __syncthreads();
+    for (int m = threadIdx.x; m + 1 < a.T; m += blockDim.x) {
+        int ok = 0;
+        if ((m & 1) == a.parity) {
+            RngKey k = a.rng;
+            k.c2 = (SITE_DBM_PT & 0xFFu) | (((uint32_t)m & 0xFFFFFFu) << 8);
+            const double u = (double)u32_to_unit_float(site_block(k, (uint32_t)p, 0).x);
+            ok = log(u) < (a.betas[m] - a.betas[m + 1]) * (E[m] - E[m + 1]);
+            if (ok) atomicAdd(a.accepted + m, 1ull);
+        }
+        acc[m] = ok;
+    }
+    __syncthreads();
+    for (int m = 0; m + 1 < a.T; ++m) {
+        if (!acc[m]) continue;
+        for (int l = 0; l <= a.L; ++l) {
+            const int n = l == 0 ? a.V : a.H[l - 1];
+            bf16_t* r0 = a.x[l] + ((size_t)m * a.M + p) * a.ld[l];
+            bf16_t* r1 = a.x[l] + ((size_t)(m + 1) * a.M + p) * a.ld[l];
+            for (int j = threadIdx.x; j < n; j += blockDim.x) { const bf16_t t = r0[j]; r0[j] = r1[j]; r1[j] = t; }
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------------------------
 struct DbmTC : Dbm<float> {
     std::vector<int> ldn;                        // leading dimension of a bf16 activation of layer idx (0 = visible)
@@ -290,7 +350,8 @@ struct DbmTC : Dbm<float> {
     // them into means / counts.  A chain of ops is therefore cut after every such op: the ops between two cuts run as one
     // program launch, the row kernel between two launches, all in stream order.  Without multinomial layers a chain is one
     // program, exactly as the ops were listed.
-    struct RowStep { int layer = -1; bf16_t* out = nullptr; float* out_f32 = nullptr; int rows = 0; bool sample = false; uint32_t site = 0, t = 0; };
+    // cut: the launch ends after this op even without a row kernel (tempered chains longer than one program)
+    struct RowStep { int layer = -1; bf16_t* out = nullptr; float* out_f32 = nullptr; int rows = 0; bool sample = false; uint32_t site = 0, t = 0; bool cut = false; };
     struct TcChain { std::vector<std::unique_ptr<TcProgram>> progs; std::vector<RowStep> after; };
     // mean-field as persistent dataflow programs of up to MF_CHUNK speculated sweeps per launch: slot history + programs
     static constexpr int MF_CHUNK = 5;
@@ -300,6 +361,15 @@ struct DbmTC : Dbm<float> {
     std::map<std::pair<int, int>, TcChain> mf_progs;                         // keyed by (rows, sweeps in the chunk)
     // committed particle sweeps as ONE persistent program: keyed by (sweeps, sampled, t0)
     std::map<std::tuple<int, int, int>, TcChain> pcd_progs;
+    // parallel tempering (bm_dbm_cfg.n_temps): T slots of M chains in rows [m M, (m+1) M) of the bf16 particle buffers; the
+    // fp32 copies v / h[i] (get_param "v", "h...") hold slot 0.  T == 1: the engine without tempering, op for op.
+    int T = 1;
+    std::vector<double> betas{1.0};
+    DevBuf<double> pt_betas;
+    DevBuf<unsigned long long> pt_accepted;      // [T - 1] swaps accepted since create
+    std::vector<long long> pt_proposed;          // [T - 1] swaps proposed since create (known on the host)
+    std::vector<DevBuf<float>> pt_pre;           // per layer [T M, H_i]: h_{i-1} W_i + c_i of the current particles
+    std::map<std::tuple<int, int, int>, TcChain> pt_progs;   // committed tempered sweeps: keyed by (sweeps, sampled, t0)
 
     // float32; Bernoulli or Gaussian visibles; Bernoulli and multinomial hidden layers in any order (the DBM's multinomial
     // particles are refused on a sharded context by init_particles)
@@ -313,16 +383,29 @@ struct DbmTC : Dbm<float> {
     bool multinomial(int i) const { return h_kinds[i] == BM_UNIT_MULTINOMIAL; }
 
     DbmTC(Ctx* c, const bm_dbm_cfg& f) : Dbm<float>(c, f) {
+        if (f.n_temps >= 1) {                    // validated by bm_dbm_create (check_pt_cfg)
+            T = f.n_temps;
+            betas.assign(f.betas, f.betas + T);
+        }
+        const size_t TM = (size_t)T * M;
         ldn.push_back(dbm_round_up(V, 64));
         for (int i = 0; i < L; ++i) ldn.push_back(dbm_round_up(Hs[i], 64));
         Wb.resize(L); WbT.resize(L); mu_b.resize(L); h_b.resize(L); h2_b.resize(L); h3_b.resize(L); Gp.resize(L);
         Xb.ensure((size_t)B * ldn[0]); recon_b.ensure((size_t)B * ldn[0]);
-        v_b.ensure((size_t)M * ldn[0]); v2_b.ensure((size_t)M * ldn[0]);
+        v_b.ensure(TM * ldn[0]); v2_b.ensure(TM * ldn[0]);
         for (DevBuf<bf16_t>* b : {&Xb, &recon_b, &v_b, &v2_b}) b->zero(ctx->stream);
+        if (T > 1) {
+            pt_betas.ensure(T);
+            BM_CUDA(cudaMemcpyAsync(pt_betas.p, betas.data(), (size_t)T * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+            pt_accepted.ensure(T - 1); pt_accepted.zero(ctx->stream);
+            pt_proposed.assign(T - 1, 0);
+            pt_pre.resize(L);
+            for (int i = 0; i < L; ++i) pt_pre[i].ensure(TM * Hs[i]);
+        }
         for (int i = 0; i < L; ++i) {
             Wb[i].ensure((size_t)size_of(i, V, Hs) * ldn[i + 1]);
             mu_b[i].ensure((size_t)B * ldn[i + 1]);
-            h_b[i].ensure((size_t)M * ldn[i + 1]); h2_b[i].ensure((size_t)M * ldn[i + 1]);
+            h_b[i].ensure(TM * ldn[i + 1]); h2_b[i].ensure(TM * ldn[i + 1]);
             for (DevBuf<bf16_t>* b : {&Wb[i], &mu_b[i], &h_b[i], &h2_b[i]}) b->zero(ctx->stream);
         }
         for (int i = 1; i < L; ++i) { WbT[i].ensure((size_t)Hs[i] * ldn[i]); WbT[i].zero(ctx->stream); }
@@ -374,13 +457,41 @@ struct DbmTC : Dbm<float> {
     }
     void widen_mu(int rows) { for (int i = 0; i < L; ++i) launch_bf16_to_f32(ctx, mu_b[i].p, ldn[i + 1], mu[i].p, Hs[i], rows, Hs[i]); }
 
+    // "v_pt" -> 0, "h_pt" -> 1, "h_pt_<i>" -> i + 1: the tempered slots 1..T-1 of a particle layer ([T-1, M, n] on the host)
+    int pt_layer(const std::string& name) const {
+        if (T <= 1) return -1;
+        if (name == "v_pt") return 0;
+        if (name == "h_pt") return 1;
+        for (int i = 1; i < L; ++i) if (name == "h_pt" + sfx(i)) return i + 1;
+        return -1;
+    }
+    void pt_param(int idx, void* host, const void* in, size_t bytes) {
+        const int n = size_of(idx, V, Hs);
+        const int rows = (T - 1) * M;
+        BM_REQUIRE(bytes == (size_t)rows * n * sizeof(float), "size mismatch for a tempered particle layer");
+        bf16_t* slots = (idx == 0 ? v_b.p : h_b[idx - 1].p) + (size_t)M * ldn[idx];
+        DevBuf<float> tmp;
+        tmp.ensure((size_t)rows * n);
+        if (in) {
+            BM_CUDA(cudaMemcpyAsync(tmp.p, in, bytes, cudaMemcpyHostToDevice, ctx->stream));
+            launch_f32_to_bf16(ctx, tmp.p, n, slots, ldn[idx], rows, n);
+        } else {
+            launch_bf16_to_f32(ctx, slots, ldn[idx], tmp.p, n, rows, n);
+            BM_CUDA(cudaMemcpyAsync(host, tmp.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        }
+        BM_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
     void set_param(const char* name, const void* host, size_t bytes) override {
+        const int pt = pt_layer(name);
+        if (pt >= 0) { pt_param(pt, nullptr, host, bytes); return; }
         widen_particles();                         // the fp32 copies become the truth for one moment
         Dbm<float>::set_param(name, host, bytes);
         narrow_state();
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
     }
     void get_param(const char* name, void* host, size_t bytes) override {
+        const int pt = pt_layer(name);
+        if (pt >= 0) { pt_param(pt, host, nullptr, bytes); return; }
         widen_particles();
         Dbm<float>::get_param(name, host, bytes);
     }
@@ -388,7 +499,32 @@ struct DbmTC : Dbm<float> {
         widen_particles();
         Dbm<float>::init_particles(seed);
         narrow_state();
+        // tempered slots: the layers' initialisers at rows row0 + M .. row0 + T M - 1 (all layers Bernoulli: U[0, 1))
+        if (T > 1) {
+            const int rows = (T - 1) * M;
+            DevBuf<float> tmp;
+            for (int idx = 0; idx <= L; ++idx) {
+                const int n = size_of(idx, V, Hs);
+                tmp.ensure((size_t)rows * n);
+                for (int r0 = 0; r0 < rows; r0 += 32768) {
+                    const int r = std::min(32768, rows - r0);
+                    particle_init_kernel<float><<<dim3(((n + 3) / 4 + 127) / 128, r), 128, 0, ctx->stream>>>(
+                        tmp.p + (size_t)r0 * n, r, n, BM_UNIT_BERNOULLI, nullptr,
+                        make_rng(seed, SITE_PARTICLE_INIT, idx, 0, particle_row0() + (uint32_t)M + (uint32_t)r0));
+                    count_launch(ctx);
+                }
+                launch_f32_to_bf16(ctx, tmp.p, n, (idx == 0 ? v_b.p : h_b[idx - 1].p) + (size_t)M * ldn[idx], ldn[idx], rows, n);
+                BM_CUDA(cudaStreamSynchronize(ctx->stream));          // tmp is reused by the next layer
+            }
+        }
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
+    void pt_counts(int64_t* accepted, int64_t* proposed) override {
+        BM_REQUIRE(T > 1, "this DBM has no tempered chains (bm_dbm_cfg.n_temps >= 2)");
+        std::vector<unsigned long long> a(T - 1);
+        BM_CUDA(cudaMemcpyAsync(a.data(), pt_accepted.p, (size_t)(T - 1) * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+        BM_CUDA(cudaStreamSynchronize(ctx->stream));
+        for (int m = 0; m + 1 < T; ++m) { accepted[m] = (int64_t)a[m]; proposed[m] = pt_proposed[m]; }
     }
 
     // ---- one fused conditional on the tensor cores -----------------------------------------------------------
@@ -472,7 +608,7 @@ struct DbmTC : Dbm<float> {
     static void cut_chain(TcChain& chain, const std::vector<TcGemm>& ops, const std::vector<RowStep>& row) {
         size_t lo = 0;
         for (size_t k = 0; k < ops.size(); ++k) {
-            if (row[k].layer < 0 && k + 1 < ops.size()) continue;
+            if (row[k].layer < 0 && !row[k].cut && k + 1 < ops.size()) continue;
             std::unique_ptr<TcProgram> p(new TcProgram());
             for (size_t j = lo; j <= k; ++j) {
                 TcGemm g = ops[j];
@@ -623,9 +759,111 @@ struct DbmTC : Dbm<float> {
         particles_f32_stale = true;
     }
 
+    // ---- parallel tempering (DESIGN.md §5.4) -------------------------------------------------------------------------
+    // k committed sweeps of all T slots: per sweep and slot the ops of particles_program with acc_scale = bias_scale = beta_m,
+    // reading and writing the slot's rows and drawing at rows row0 + m M + p (TcGemm::row_off).  Dependencies stay inside a
+    // slot, and slot m runs on CTA pairs of its own (as the members of a training group), so the slots' ops run side by side.
+    // Ops are listed sweep by sweep, layer by layer, slot by slot.  A chain longer than one program is cut between sweeps; a
+    // single sweep of more than TC_PROGRAM_OPS ops (many slots) is cut every TC_PROGRAM_OPS ops, the kernel boundary then
+    // ordering whatever depends across the cut.  Sweep s draws at t = t0 + s + 1.
+    void particles_program_pt(int n_steps, bool sample, uint64_t seed, uint32_t tick, int t0) {
+        TcChain& chain = pt_progs[std::make_tuple(n_steps, sample ? 1 : 0, t0)];
+        std::vector<bf16_t*> cur(L), nxt(L);
+        for (int i = 0; i < L; ++i) { cur[i] = h_b[i].p; nxt[i] = h2_b[i].p; }
+        bf16_t* vc = v_b.p; bf16_t* vn = v2_b.p;
+        if (chain.progs.empty()) {
+            auto rows_of = [&](bf16_t* base, int idx, int m) { return base + (size_t)m * M * ldn[idx]; };
+            const int total_pairs = ctx->sm_count / 2;
+            int per = 0;                                               // CTA pairs of a slot: its largest op's units, at most 1/T of the grid
+            std::vector<TcGemm> ops;
+            std::vector<RowStep> row;
+            std::vector<int> last_vis(T, -1);
+            std::vector<std::vector<int>> last_h(T, std::vector<int>(L, -1)), this_h = last_h;
+            const int sweep_ops = T * (L + 1);
+            const int sweeps_per_launch = std::max(1, TC_PROGRAM_OPS / sweep_ops);
+            for (int s = 0; s < n_steps; ++s) {
+                const uint32_t tstep = (uint32_t)(t0 + s + 1);
+                for (int i = 0; i <= L; ++i)
+                    for (int m = 0; m < T; ++m) {
+                        const float b = (float)betas[m];
+                        TcGemm g;
+                        if (i < L) {
+                            const bf16_t* below = i == 0 ? rows_of(vc, 0, m) : rows_of(nxt[i - 1], i, m);
+                            const bf16_t* above = (i + 1 < L) ? rows_of(cur[i + 1], i + 2, m) : nullptr;
+                            g = hidden_gemm(i, below, above, rows_of(nxt[i], i + 1, m), sample && sample_h[i], M, b, b,
+                                            make_rng(0, SITE_DBM_H + i, tstep, 0, 0));
+                            const int below_op = i == 0 ? last_vis[m] : this_h[m][i - 1];
+                            if (below_op >= 0) { g.dep[g.n_deps] = below_op; g.dep_all[g.n_deps] = false; ++g.n_deps; }
+                            if (above && last_h[m][i + 1] >= 0) { g.dep[g.n_deps] = last_h[m][i + 1]; g.dep_all[g.n_deps] = false; ++g.n_deps; }
+                            this_h[m][i] = (int)ops.size();
+                        } else {
+                            g = visible_gemm(rows_of(nxt[0], 1, m), rows_of(vn, 0, m), sample && sample_vis, M, make_rng(0, SITE_DBM_V, tstep, 0, 0));
+                            g.acc_scale = b; g.bias_scale = b;
+                            g.dep[0] = this_h[m][0]; g.dep_all[0] = false; g.n_deps = 1;
+                            last_vis[m] = (int)ops.size();
+                        }
+                        g.row_off = (uint32_t)m * (uint32_t)M;
+                        g.lane = LANE_CHAIN;
+                        g.pair_begin = m;                                      // the slot, until the pair ranges are known
+                        if (s == 0) per = std::max(per, tc_plan_units(ctx, g));
+                        ops.push_back(g);
+                        RowStep st;
+                        if (sweep_ops <= TC_PROGRAM_OPS)                       // a launch ends with a whole sweep
+                            st.cut = (i == L && m == T - 1 && (s + 1) % sweeps_per_launch == 0);
+                        else                                                   // or with TC_PROGRAM_OPS ops of a long sweep
+                            st.cut = (ops.size() % TC_PROGRAM_OPS == 0) || (i == L && m == T - 1);
+                        row.push_back(st);
+                    }
+                for (int m = 0; m < T; ++m) last_h[m] = this_h[m];
+                std::swap(cur, nxt); std::swap(vc, vn);
+            }
+            per = std::max(1, std::min(total_pairs / T, per));
+            for (TcGemm& g : ops) { g.pair_begin = (g.pair_begin * per) % (total_pairs - per + 1); g.pair_count = per; }
+            cut_chain(chain, ops, row);
+        } else if (n_steps % 2) {
+            std::swap(cur, nxt); std::swap(vc, vn);
+        }
+        run_chain(chain, make_rng(seed, 0, 0, tick, particle_row0()), seed, tick);
+        const size_t TM = (size_t)T * M;
+        for (int i = 0; i < L; ++i)
+            if (cur[i] != h_b[i].p)
+                BM_CUDA(cudaMemcpyAsync(h_b[i].p, cur[i], TM * ldn[i + 1] * sizeof(bf16_t), cudaMemcpyDeviceToDevice, ctx->stream));
+        if (vc != v_b.p) BM_CUDA(cudaMemcpyAsync(v_b.p, vc, TM * ldn[0] * sizeof(bf16_t), cudaMemcpyDeviceToDevice, ctx->stream));
+        particles_f32_stale = true;
+    }
+    // One swap round over the committed particles: the energies' products (one raw fp32 op per weight matrix over all T M rows),
+    // then dbm_pt_swap_kernel.  The proposed pairs alternate with the call's tick: (m, m+1) with m = tick (mod 2).
+    void pt_swap_round(uint64_t seed, uint32_t tick) {
+        const int TM = T * M;
+        PtSwapArgs a;
+        memset(&a, 0, sizeof(a));
+        a.L = L; a.T = T; a.M = M; a.V = V;
+        a.x[0] = v_b.p; a.ld[0] = ldn[0];
+        for (int i = 0; i < L; ++i) {
+            const int in = size_of(i, V, Hs);
+            linear_tc(i == 0 ? v_b.p : h_b[i - 1].p, ldn[i], TM, in, Wb[i].p, in, Hs[i], ldn[i + 1], true, Hs[i], hb[i].p, pt_pre[i].p);
+            a.H[i] = Hs[i]; a.x[i + 1] = h_b[i].p; a.ld[i + 1] = ldn[i + 1]; a.P[i] = pt_pre[i].p;
+        }
+        a.vb = vb.p; a.betas = pt_betas.p;
+        a.parity = (int)(tick & 1u);
+        a.rng = make_rng(seed, SITE_DBM_PT, 0, tick, particle_row0());
+        a.accepted = pt_accepted.p;
+        dbm_pt_swap_kernel<<<M, 256, (size_t)T * (sizeof(double) + sizeof(int)), ctx->stream>>>(a);
+        count_launch(ctx);
+        for (int m = a.parity; m + 1 < T; m += 2) pt_proposed[m] += M;
+        particles_f32_stale = true;
+    }
+
     // committed sweeps that fit in one program run as that program; uncommitted runs (the second half of sample_v) and
-    // longer chains take one launch per op
+    // longer chains take one launch per op.  With tempering, a committed update runs every slot (cut into launches between
+    // sweeps when it is long) and ends with a swap round; an uncommitted run only needs slot 0, whose output it is.
     void particles_tc(int n_steps, bool sample, uint64_t seed, uint32_t tick, int t0, bool commit, bf16_t** v_final) {
+        if (commit && T > 1) {
+            if (n_steps >= 1) particles_program_pt(n_steps, sample, seed, tick, t0);
+            pt_swap_round(seed, tick);
+            if (v_final) *v_final = v_b.p;
+            return;
+        }
         if (commit && n_steps >= 1 && n_steps * (L + 1) <= TC_PROGRAM_OPS) {
             particles_program(n_steps, sample, seed, tick, t0);
             if (v_final) *v_final = v_b.p;

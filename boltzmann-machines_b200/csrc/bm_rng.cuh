@@ -20,6 +20,7 @@ enum Site : uint32_t {
     SITE_DROPOUT = 0, SITE_H0 = 1, SITE_V = 2, SITE_H = 3, SITE_PLL = 4,
     SITE_MULTINOMIAL_FE = 5, SITE_PARTICLE_INIT = 6, SITE_AIS_INIT = 7,
     SITE_AIS_V = 8, SITE_AIS_H2 = 9, SITE_AIS_H1 = 10, SITE_DBM_V = 11, SITE_CRBM_Y = 12, SITE_CRBM_Y0 = 13,
+    SITE_DBM_PT = 14,        // parallel tempering: the swap decision of pair (m, m+1) at t = m, column 0 of the particle's row
     SITE_DBM_H = 16
 };
 

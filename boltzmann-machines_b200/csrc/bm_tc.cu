@@ -924,7 +924,7 @@ tc_program_kernel(const __grid_constant__ TcLaunch L) {
             c.p.out_f32 = ph->out_f32; c.p.ld_f32 = ph->ld_f32; c.p.split_stride = ph->split_stride;
             c.p.ais_a = ph->ais_a; c.p.ais_b = ph->ais_b; c.p.ais_next = ph->ais_next; c.p.ais_lin = ph->ais_lin; c.p.ais_logw = ph->ais_logw;
             c.p.ais_ct = ph->ais_b - ph->ais_a; c.p.ais_cd = ph->ais_next - 0.5f * (ph->ais_a + ph->ais_b);
-            c.rng.k0 = ph->k0; c.rng.k1 = ph->k1; c.rng.tick = L.tick + ph->tick_off; c.rng.row0 = L.row0; c.rng.c2 = ph->rng_c2;
+            c.rng.k0 = ph->k0; c.rng.k1 = ph->k1; c.rng.tick = L.tick + ph->tick_off; c.rng.row0 = L.row0 + ph->row_off; c.rng.c2 = ph->rng_c2;
             c.m0 = (u.m_group * CL + crank) * BM + c.r0;
             c.n_blk = u.n_blk; c.split = u.split;
             switch (ph->mode) {
@@ -1097,7 +1097,7 @@ static void fill_phase(Ctx* ctx, const TcGemm& g, int cluster, TcPhase& ph) {
     p.k0 = g.rng.k0; p.k1 = g.rng.k1;
     p.rng_c2 = g.rng.c2;
     p.ais_kind = g.ais_kind; p.ais_a = g.ais_a; p.ais_b = g.ais_b; p.ais_next = g.ais_next; p.ais_lin = g.ais_lin;
-    p.ais_logw = g.ais_logw; p.tick_off = g.tick_off;
+    p.ais_logw = g.ais_logw; p.tick_off = g.tick_off; p.row_off = g.row_off;
     if (g.ais_kind == 1)
         BM_REQUIRE(!g.sigma && !g.noise_sigma && g.act == ACT_LINEAR && !g.out_mean_bf && !g.out_f32 && g.splits <= 1 &&
                    g.acc_scale == 1.f && g.bias_scale == 1.f && (g.sample == SMP_NONE || g.sample == SMP_BERNOULLI),

@@ -63,6 +63,7 @@ struct TcGemm {
     float ais_a = 0.f, ais_b = 0.f, ais_next = 0.f, ais_lin = 0.f;
     double* ais_logw = nullptr;
     uint32_t tick_off = 0;
+    uint32_t row_off = 0;             // draws of row r come from row rng.row0 + row_off + r (slot m of a tempered ladder: m * rows)
 };
 enum : int { LANE_CHAIN = 0, LANE_SPARE = 1, LANE_ALL = 2 };
 

@@ -52,6 +52,7 @@ struct TcPhaseLite {
     float ais_a, ais_b, ais_next, ais_lin;
     double* ais_logw;
     uint32_t tick_off;               // added to the launch's tick for this op's draws
+    uint32_t row_off;                // added to the launch's first row for this op's draws (tempered particle slots)
 };
 struct alignas(64) TcPhase {
     CUtensorMap tmA[2], tmB[2];      // read by the TMA unit from global / parameter memory

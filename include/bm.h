@@ -199,13 +199,22 @@ typedef struct bm_dbm_cfg {
     const double* sparsity_target;
     const double* sparsity_cost;
     const double* sigma;             /* [n_visible] for a gaussian visible layer, else NULL */
+    /* Parallel tempering of the persistent chains (Desjardins et al., AISTATS 2010).  0 / NULL: off.  Otherwise n_temps
+     * inverse temperatures betas[0] = 1 > betas[1] > ... > betas[n_temps-1] >= 0; slot m holds n_particles chains swept at
+     * betas[m] (conditionals sigmoid(beta (x + b))), and every committed particle update ends with one round of swaps
+     * between neighbouring slots (DESIGN.md §5.4).  Slot 0 is the chain without tempering: gradients, column sums,
+     * sample_v and the names "v" / "h..." read it.  BM_EUNSUPPORTED: the fp32 / fp64 engines, gaussian visibles, multinomial
+     * hidden layers, a context with a communicator; BM_EINVAL: a malformed ladder, sample_v == 0 or any sample_h == 0. */
+    int32_t n_temps;
+    const double* betas;
 } bm_dbm_cfg;
 
 int  bm_dbm_create(bm_ctx* ctx, const bm_dbm_cfg* cfg, bm_dbm** out);      /* DBM._make_tf_model, dbm.py:761-769 */
 void bm_dbm_destroy(bm_dbm* dbm);
 /* variables by TF-uniquified name (dbm.py:294-383, dbm_mnist.py:367-371): "vb", "W", "W_1", "hb", "hb_1",
  * "dvb", "dW"..., "dhb"..., "mu"... [batch_size,H_i], "q_means"..., "mu_means"..., particles "v" [n_particles,V],
- * "h", "h_1"... [n_particles,H_i] */
+ * "h", "h_1"... [n_particles,H_i]; with parallel tempering also the tempered slots 1..n_temps-1 "v_pt"
+ * [n_temps-1,n_particles,V], "h_pt", "h_pt_1"... [n_temps-1,n_particles,H_i] */
 int  bm_dbm_set_param(bm_dbm* dbm, const char* name, const void* host, size_t bytes);
 int  bm_dbm_get_param(bm_dbm* dbm, const char* name, void* host, size_t bytes);
 /* persistent particles <- the layers' own random initialisers (dbm.py:362-383) */
@@ -229,6 +238,9 @@ int  bm_dbm_ais(bm_dbm* dbm, int32_t n_runs, int32_t n_betas, int32_t n_gibbs_st
  * themselves (one process driving several GPUs; more runs than fit in memory at once) */
 int  bm_dbm_ais_rows(bm_dbm* dbm, int32_t n_runs, int32_t n_betas, int32_t n_gibbs_steps, uint64_t seed, uint32_t first_run,
                      double* logZ);
+/* parallel tempering: swaps accepted / proposed between slots m and m+1 since create, n_temps-1 entries each (BM_EINVAL
+ * without tempering) */
+int  bm_dbm_pt_counts(bm_dbm* dbm, int64_t* accepted, int64_t* proposed);
 
 /* ---- test hook: the raw tensor-core GEMM (no counterpart in the reference) -----------------
  * C[M,N] (fp32) = A * B^T (+/- A2 * B2^T), operands given as host fp32 and rounded to bf16.
