@@ -11,3 +11,5 @@ from . import rbm
 from .rbm import BaseRBM, BernoulliRBM, MultinomialRBM, GaussianRBM, ClassificationRBM, logit_mean, fit_many
 from . import dbm
 from .dbm import DBM
+from . import class_dbm
+from .class_dbm import ClassificationDBM

@@ -31,6 +31,7 @@ EXPORTS = (
     'bm_dbm_create', 'bm_dbm_destroy', 'bm_dbm_set_param', 'bm_dbm_get_param', 'bm_dbm_init_particles',
     'bm_dbm_train_step', 'bm_dbm_val_metrics', 'bm_dbm_transform', 'bm_dbm_reconstruct', 'bm_dbm_log_proba',
     'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows', 'bm_dbm_pt_counts', 'bm_debug_dbm_multinomial_rows',
+    'bm_dbm_train_step_labeled', 'bm_dbm_predict_proba',
     'bm_crbm_create', 'bm_crbm_destroy', 'bm_crbm_set_param', 'bm_crbm_get_param', 'bm_crbm_init_weights',
     'bm_crbm_train_step', 'bm_crbm_predict_proba', 'bm_crbm_transform',
     'bm_rbm_group_create', 'bm_rbm_group_destroy', 'bm_rbm_group_train_epoch', 'bm_rbm_group_train_epoch_u8',
@@ -70,6 +71,7 @@ class DbmCfg(C.Structure):
         ('sigma', C.POINTER(C.c_double)),
         ('n_temps', C.c_int32),
         ('betas', C.POINTER(C.c_double)),
+        ('n_classes', C.c_int32),
     ]
 
 
@@ -162,6 +164,8 @@ def load_library(path=None):
         'bm_dbm_ais': [vp, i32, i32, i32, u64, vp],
         'bm_dbm_ais_rows': [vp, i32, i32, i32, u64, u32, vp],
         'bm_dbm_pt_counts': [vp, vp, vp],
+        'bm_dbm_train_step_labeled': [vp, vp, vp, i32, dbl, dbl, i32, u64, u32, i32, C.POINTER(dbl)],
+        'bm_dbm_predict_proba': [vp, vp, i32, vp],
         'bm_debug_dbm_multinomial_rows': [vp, vp, i32, i32, dbl, i32, u64, u32, u32, u32, vp, vp, vp, vp],
         'bm_crbm_create': [vp, C.POINTER(CrbmCfg), C.POINTER(vp)],
         'bm_crbm_set_param': [vp, C.c_char_p, vp, sz], 'bm_crbm_get_param': [vp, C.c_char_p, vp, sz],
@@ -793,11 +797,17 @@ class CudaDBM(object):
         if self.pt_betas is not None:
             c.n_temps = len(self.pt_betas)
             c.betas = self.pt_betas.ctypes.data_as(C.POINTER(C.c_double))
+        # classification DBM: a one-of-n_classes label layer above the last hidden layer (0: none; tensor-core engine only)
+        self.C = int(cfg.get('n_classes', 0) or 0)
+        c.n_classes = self.C
+        if self.C:
+            self.compute = cfg.get('compute') or 'bf16'
+            c.compute = COMPUTE[self.compute]
         h = C.c_void_p()
         rc = self._lib.bm_dbm_create(self.ctx.handle, C.byref(c), C.byref(h))
         if rc in (-1, -5):
             err = self._lib.bm_last_error().decode('utf-8', 'replace')
-            if err.startswith('parallel tempering'):
+            if err.startswith('parallel tempering') or err.startswith('classification DBM'):
                 raise (NotImplementedError if rc == -5 else ValueError)('libbm: ' + err)
         check(rc)
         self.handle = h
@@ -812,6 +822,10 @@ class CudaDBM(object):
             self._shapes['v_pt'] = (self.T - 1, self.M, self.V)
             for i in range(self.L):
                 self._shapes['h_pt' + _sfx(i)] = (self.T - 1, self.M, self.Hs[i])
+        if self.C:
+            Cn, H = self.C, self.Hs[-1]
+            self._shapes.update({'U': (Cn, H), 'dU': (Cn, H), 'yb': (Cn,), 'dyb': (Cn,), 'y': (self.M, Cn),
+                                 'mu_y': (self.B, Cn)})
         self._out2 = (C.c_double * 2)()
 
     def pt_counts(self):
@@ -844,11 +858,26 @@ class CudaDBM(object):
             raise ValueError('batch has shape {0}, expected (rows, {1})'.format(X.shape, self.V))
         return X
 
-    def train_step(self, X, lr, momentum, k, seed, tick, metrics=()):
+    def train_step(self, X, lr, momentum, k, seed, tick, metrics=(), labels=None):
+        """``labels`` (classification DBMs): [rows] ints in [-1, n_classes), -1 for an unlabelled row."""
         X = self._batch(X)
-        check(self._lib.bm_dbm_train_step(self.handle, X.ctypes.data, X.shape[0], lr, momentum, int(k), int(seed), int(tick),
-                                          1 if metrics else 0, self._out2))
+        if labels is None:
+            check(self._lib.bm_dbm_train_step(self.handle, X.ctypes.data, X.shape[0], lr, momentum, int(k), int(seed),
+                                              int(tick), 1 if metrics else 0, self._out2))
+        else:
+            y = np.ascontiguousarray(labels, dtype=np.int32).reshape(-1)
+            if y.shape[0] != X.shape[0]:
+                raise ValueError('{0} labels for {1} rows'.format(y.shape[0], X.shape[0]))
+            check(self._lib.bm_dbm_train_step_labeled(self.handle, X.ctypes.data, y.ctypes.data, X.shape[0], lr, momentum,
+                                                      int(k), int(seed), int(tick), 1 if metrics else 0, self._out2))
         return {'msre': float(self._out2[0]), 'n_mf_updates': float(self._out2[1])} if metrics else None
+
+    def predict_proba(self, X):
+        """classification DBMs: softmax(yb + mu_L U^T) [rows, n_classes] (float32) after the E-step with y free"""
+        X = self._batch(X)
+        out = np.empty((X.shape[0], self.C), dtype=np.float32)
+        check(self._lib.bm_dbm_predict_proba(self.handle, X.ctypes.data, X.shape[0], out.ctypes.data))
+        return out
 
     def val_metrics(self, X, k, seed, tick):
         X = self._batch(X)

@@ -198,6 +198,10 @@ struct DbmBase {
     virtual void ais(int n_runs, int n_betas, int k, uint64_t seed, double* out) = 0;
     virtual void ais_rows(int n_runs, int n_betas, int k, uint64_t seed, uint32_t first_run, double* out) = 0;
     virtual void pt_counts(int64_t*, int64_t*) { throw Error(BM_EINVAL, "this DBM has no tempered chains (bm_dbm_cfg.n_temps)"); }
+    virtual void train_step_labeled(const void*, const int32_t*, int, double, double, int, uint64_t, uint32_t, int, double*) {
+        throw Error(BM_EINVAL, "this DBM has no label layer (bm_dbm_cfg.n_classes)");
+    }
+    virtual void predict_proba(const void*, int, float*) { throw Error(BM_EINVAL, "this DBM has no label layer (bm_dbm_cfg.n_classes)"); }
 };
 
 // Parallel tempering (bm_dbm_cfg.n_temps / betas): what the engines refuse before anything is allocated.  0 / NULL is off.
@@ -700,6 +704,7 @@ struct Dbm : DbmBase {
 
 #include "bm_dbm_tc.cuh"     // DbmTC: the same engine with every GEMM on the tensor cores (opt-in)
 #include "bm_crbm_tc.cuh"    // ClassRbmTC: the classification RBM, a DbmTC of shape x - h - label (bm_crbm_*)
+#include "bm_cdbm_tc.cuh"    // ClassDbmTC: the classification DBM, a DbmTC with a label layer on top (bm_dbm_cfg.n_classes)
 
 using namespace bm;
 
@@ -713,6 +718,8 @@ int bm_dbm_create(bm_ctx* hctx, const bm_dbm_cfg* cfg, bm_dbm** out) {
     BM_REQUIRE(cfg->n_hiddens && cfg->h_kinds && cfg->sample_h && cfg->sparsity_target && cfg->sparsity_cost, "missing per-layer arrays");
     BM_REQUIRE(cfg->n_particles > 0 && cfg->batch_size > 0, "n_particles and batch_size must be positive");
     BM_REQUIRE(cfg->v_kind != BM_UNIT_GAUSSIAN || cfg->sigma, "gaussian visible layer needs sigma");
+    BM_REQUIRE(cfg->n_classes >= 0 && cfg->n_classes != 1, "classification DBM: n_classes must be 0 (no label layer) or at least 2");
+    if (cfg->n_classes >= 2) ClassDbmTC::check_cfg(ctx, *cfg);      // then n_temps <= 1: at most [1.0], no tempering
     check_pt_cfg(ctx, *cfg);
     if (cfg->n_temps >= 1 && !DbmTC::supports(*cfg)) throw Error(BM_EUNSUPPORTED, "parallel tempering: the model does not run on the tensor-core engine");
     BM_CUDA(cudaSetDevice(ctx->device));
@@ -720,7 +727,9 @@ int bm_dbm_create(bm_ctx* hctx, const bm_dbm_cfg* cfg, bm_dbm** out) {
     // cores; every other combination keeps the storage-precision CUDA-core engine (as bm_rbm_create does for unit kinds the
     // tensor-core epilogue does not implement)
     DbmBase* d;
-    if (cfg->dtype == BM_DTYPE_F64) d = new Dbm<double>(ctx, *cfg);
+    CdbmShape s;
+    if (cfg->n_classes >= 2) d = new ClassDbmTC(ctx, *cfg, s);
+    else if (cfg->dtype == BM_DTYPE_F64) d = new Dbm<double>(ctx, *cfg);
     else if (cfg->compute == BM_COMPUTE_BF16 && DbmTC::supports(*cfg)) d = new DbmTC(ctx, *cfg);
     else d = new Dbm<float>(ctx, *cfg);
     *out = reinterpret_cast<bm_dbm*>(d);
@@ -748,6 +757,15 @@ int bm_dbm_train_step(bm_dbm* h, const void* X, int32_t rows, double lr, double 
     BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(X, "null batch");
     DBM(h)->train_step(X, rows, lr, momentum, k, seed, tick, want_metrics, out2);
     BM_API_END
+}
+int bm_dbm_train_step_labeled(bm_dbm* h, const void* X, const int32_t* labels, int32_t rows, double lr, double momentum,
+                              int32_t n_gibbs_steps, uint64_t seed, uint32_t tick, int32_t want_metrics, double* out2) {
+    BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(X && labels, "null argument");
+    DBM(h)->train_step_labeled(X, labels, rows, lr, momentum, n_gibbs_steps, seed, tick, want_metrics, out2);
+    BM_API_END
+}
+int bm_dbm_predict_proba(bm_dbm* h, const void* X, int32_t rows, float* out) {
+    BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(X && out, "null argument"); DBM(h)->predict_proba(X, rows, out); BM_API_END
 }
 int bm_dbm_val_metrics(bm_dbm* h, const void* X, int32_t rows, int32_t k, uint64_t seed, uint32_t tick, double* out2) {
     BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(X && out2, "null argument"); DBM(h)->val_metrics(X, rows, k, seed, tick, out2); BM_API_END

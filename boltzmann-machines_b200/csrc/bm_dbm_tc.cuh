@@ -123,6 +123,25 @@ __global__ void __launch_bounds__(256) dbm_multinomial_rows_kernel(const float* 
         if (out_f32) out_f32[(size_t)r * ldf + c] = k;
     }
 }
+// The label clamp of a classification DBM (DESIGN.md §5.7): rows r < rows whose label t = labels[r] is >= 0 get the one-hot
+// e_t in columns [0, cols) of `n_slots` bf16 buffers [rows, ld] spaced `slot_stride` apart (slot = blockIdx.y); rows labelled -1
+// are left as they are.  One warp per row.
+__global__ void cdbm_clamp_labels_kernel(const int* __restrict__ labels, int rows, int cols, bf16_t* __restrict__ out, int ld,
+                                         size_t slot_stride) {
+    const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (r >= rows) return;
+    const int t = labels[r];
+    if (t < 0) return;
+    bf16_t* row = out + (size_t)blockIdx.y * slot_stride + (size_t)r * ld;
+    for (int c = lane; c < cols; c += 32) row[c] = __float2bfloat16_rn(c == t ? 1.f : 0.f);
+}
+void launch_cdbm_clamp_labels(Ctx* ctx, const int* labels, int rows, int cols, bf16_t* out, int ld, int n_slots = 1,
+                              size_t slot_stride = 0) {
+    if (rows <= 0 || n_slots <= 0) return;
+    cdbm_clamp_labels_kernel<<<dim3((rows + 7) / 8, n_slots), 256, 0, ctx->stream>>>(labels, rows, cols, out, ld, slot_stride);
+    count_launch(ctx);
+}
+
 static inline size_t dbm_multinomial_smem(int cols, bool draws) {
     return ((size_t)cols * sizeof(float) + 7) / 8 * 8 + (draws ? (size_t)cols * (sizeof(double) + sizeof(int)) : 0);
 }
@@ -351,14 +370,25 @@ struct DbmTC : Dbm<float> {
     // program launch, the row kernel between two launches, all in stream order.  Without multinomial layers a chain is one
     // program, exactly as the ops were listed.
     // cut: the launch ends after this op even without a row kernel (tempered chains longer than one program)
-    struct RowStep { int layer = -1; bf16_t* out = nullptr; float* out_f32 = nullptr; int rows = 0; bool sample = false; uint32_t site = 0, t = 0; bool cut = false; };
+    // clamp: after the row kernel, the rows of `out` labelled >= 0 in this device array are set to their one-hot label
+    struct RowStep { int layer = -1; bf16_t* out = nullptr; float* out_f32 = nullptr; int rows = 0; bool sample = false; uint32_t site = 0, t = 0; bool cut = false;
+                     const int* clamp = nullptr; };
     struct TcChain { std::vector<std::unique_ptr<TcProgram>> progs; std::vector<RowStep> after; };
     // mean-field as persistent dataflow programs of up to MF_CHUNK speculated sweeps per launch: slot history + programs
     static constexpr int MF_CHUNK = 5;
     int mf_chunk = 0;                            // MF_CHUNK, clamped by max_mf and by TC_PROGRAM_OPS, at least 1
     std::vector<DevBuf<bf16_t>> hist;            // per layer: (mf_chunk + 2) slots of [B, ldn[i+1]]
     DevBuf<unsigned int> mf_flags;
-    std::map<std::pair<int, int>, TcChain> mf_progs;                         // keyed by (rows, sweeps in the chunk)
+    std::map<std::tuple<int, int, int>, TcChain> mf_progs;                   // keyed by (rows, sweeps in the chunk, mf_clamp)
+    // The label layer of a classification DBM (ClassDbmTC, DESIGN.md §5.7) is the top layer L - 1.  Its E-step values of rows
+    // labelled t >= 0 (mf_labels, device) are the one-hot e_t in every history slot:
+    //   CLAMP_NONE  every value is free: the plain engine, op for op
+    //   CLAMP_ROWS  a mixed batch: the top layer's row kernel is followed by the clamp of the labelled rows
+    //   CLAMP_ALL   every row labelled: the top layer's ops are not run; the ops below it read the one-hot slots
+    enum { CLAMP_NONE = 0, CLAMP_ROWS = 1, CLAMP_ALL = 2 };
+    int mf_clamp = CLAMP_NONE;
+    const int* mf_labels = nullptr;
+    bool top_is_label = false;                   // the top layer's bias takes the plain momentum update, no sparsity term
     // committed particle sweeps as ONE persistent program: keyed by (sweeps, sampled, t0)
     std::map<std::tuple<int, int, int>, TcChain> pcd_progs;
     // parallel tempering (bm_dbm_cfg.n_temps): T slots of M chains in rows [m M, (m+1) M) of the bf16 particle buffers; the
@@ -632,6 +662,7 @@ struct DbmTC : Dbm<float> {
             if (st.layer >= 0)
                 multinomial_rows(st.layer, st.rows, st.out, st.out_f32, st.sample,
                                  st.sample ? make_rng(seed, st.site, st.t, tick, particle_row0()) : RngKey{});
+            if (st.clamp) launch_cdbm_clamp_labels(ctx, st.clamp, st.rows, Hs[st.layer], st.out, ldn[st.layer + 1]);
         }
     }
 
@@ -644,39 +675,52 @@ struct DbmTC : Dbm<float> {
     // sweep-by-sweep loop.  Slots: 0 = S_{a-1}, 1 = S_a, 2.. = S_{a+1}...; test t of the chunk compares slots t+1 and t.
     bf16_t* slot(int i, int s) { return hist[i].p + (size_t)s * B * ldn[i + 1]; }
     int mean_field_tc(int rows) {
+        const int top = L - 1;
+        const bool skip_top = mf_clamp == CLAMP_ALL;                         // the label layer's ops are not run
+        if (mf_clamp != CLAMP_NONE) {        // labelled rows: e_t in the previous value and in every history slot
+            launch_cdbm_clamp_labels(ctx, mf_labels, rows, Hs[top], mu_b[top].p, ldn[top + 1]);
+            launch_cdbm_clamp_labels(ctx, mf_labels, rows, Hs[top], hist[top].p, ldn[top + 1], mf_chunk + 2, (size_t)B * ldn[top + 1]);
+        }
         for (int i = 0; i < L; ++i) {                                        // approximate-inference pass -> slot 0
             const bf16_t* below = i == 0 ? Xb.p : slot(i - 1, 0);
             const float sc = (i == 0 || i < L - 1) ? 2.f : 1.f;
-            hidden_tc(i, below, nullptr, slot(i, 0), false, rows, sc, 1.f, RngKey{});
+            if (!(skip_top && i == top)) hidden_tc(i, below, nullptr, slot(i, 0), false, rows, sc, 1.f, RngKey{});
+            if (mf_clamp == CLAMP_ROWS && i == top) launch_cdbm_clamp_labels(ctx, mf_labels, rows, Hs[top], slot(top, 0), ldn[top + 1]);
             BM_CUDA(cudaMemcpyAsync(slot(i, 1), mu_b[i].p, (size_t)rows * ldn[i + 1] * sizeof(bf16_t), cudaMemcpyDeviceToDevice, ctx->stream));
         }
         int a = 0, result_slot = 1;
         bool done = false;
         while (!done && a < max_mf) {
             const int c = std::min(mf_chunk, max_mf - a);
-            TcChain& chain = mf_progs[std::make_pair(rows, c)];
+            TcChain& chain = mf_progs[std::make_tuple(rows, c, mf_clamp)];
             if (chain.progs.empty()) {
                 std::vector<TcGemm> ops;
                 std::vector<RowStep> row;
-                for (int s = 1; s <= c; ++s)                                 // sweep s: slot s -> slot s + 1
+                std::vector<int> prev(L, -1), cur(L, -1);                    // op indices of each layer in the last / this sweep
+                for (int s = 1; s <= c; ++s) {                               // sweep s: slot s -> slot s + 1
                     for (int i = 0; i < L; ++i) {
+                        if (skip_top && i == top) continue;
                         const bf16_t* below = i == 0 ? Xb.p : slot(i - 1, s + 1);
                         const bf16_t* above = (i + 1 < L) ? slot(i + 1, s) : nullptr;
                         TcGemm g = hidden_gemm(i, below, above, slot(i, s + 1), false, rows, 1.f, 1.f, RngKey{});
-                        const int self = (int)ops.size();
-                        if (i > 0) { g.dep[g.n_deps] = self - 1; g.dep_all[g.n_deps] = false; ++g.n_deps; }           // layer i-1, this sweep
-                        if (above && s > 1) { g.dep[g.n_deps] = self - L + 1; g.dep_all[g.n_deps] = false; ++g.n_deps; } // layer i+1, previous sweep
+                        if (i > 0) { g.dep[g.n_deps] = cur[i - 1]; g.dep_all[g.n_deps] = false; ++g.n_deps; }                // layer i-1, this sweep
+                        if (above && prev[i + 1] >= 0) { g.dep[g.n_deps] = prev[i + 1]; g.dep_all[g.n_deps] = false; ++g.n_deps; } // layer i+1, previous sweep
                         g.lane = LANE_CHAIN;
+                        cur[i] = (int)ops.size();
                         ops.push_back(g);
                         RowStep st;
                         if (multinomial(i)) { st.layer = i; st.out = slot(i, s + 1); st.rows = rows; }
+                        if (mf_clamp == CLAMP_ROWS && i == top) st.clamp = mf_labels;
                         row.push_back(st);
                     }
+                    prev = cur;
+                }
                 cut_chain(chain, ops, row);
             }
             run_chain(chain, RngKey{}, 0, 0);
             BM_CUDA(cudaMemsetAsync(mf_flags.p, 0, (size_t)c * sizeof(unsigned int), ctx->stream));
             for (int i = 0; i < L; ++i) {
+                if (skip_top && i == top) continue;                          // every slot holds the same one-hot rows
                 mf_chunk_diffs_kernel<<<dim3((unsigned)(ctx->sm_count / 2), c), 256, 0, ctx->stream>>>(hist[i].p, (size_t)B * ldn[i + 1], ldn[i + 1], rows, Hs[i], mf_flags.p);
                 count_launch(ctx);
             }
@@ -962,10 +1006,15 @@ struct DbmTC : Dbm<float> {
         count_launch(ctx);
         for (int i = 0; i < L; ++i) {
             const int in = size_of(i, V, Hs), H = Hs[i];
-            BM_REQUIRE(i < H, "the reference's sparsity update indexes element i of layer i's unit vector");
-            dbm_sparsity_bias_kernel<float><<<(H + 255) / 256, 256, 0, ctx->stream>>>(
-                H, i, musum[i].p, hsum[i].p, rows_g, Mp, qm[i].p, mm[i].p, pen[i].p, hb[i].p, dhb[i].p,
-                (float)damping, (float)sp_cost[i], (float)sp_target[i], (float)lr, (float)mom);
+            if (top_is_label && i == L - 1) {      // yb: sum q(y) / rows - sum y / M, the plain momentum update (pen stays 0)
+                dbm_vbias_kernel<float><<<(H + 255) / 256, 256, 0, ctx->stream>>>(H, musum[i].p, hsum[i].p, rows_g, Mp, hb[i].p, dhb[i].p,
+                                                                                 (float)lr, (float)mom);
+            } else {
+                BM_REQUIRE(i < H, "the reference's sparsity update indexes element i of layer i's unit vector");
+                dbm_sparsity_bias_kernel<float><<<(H + 255) / 256, 256, 0, ctx->stream>>>(
+                    H, i, musum[i].p, hsum[i].p, rows_g, Mp, qm[i].p, mm[i].p, pen[i].p, hb[i].p, dhb[i].p,
+                    (float)damping, (float)sp_cost[i], (float)sp_target[i], (float)lr, (float)mom);
+            }
             count_launch(ctx);
             launch_weight_update<float>(ctx, G[i].p, H, 1.f, W[i].p, dW[i].p, in, H, pen[i].p, (float)l2, (float)lr, (float)mom, nullptr, 0);
             colnorm_kernel<float><<<(H + 31) / 32, dim3(32, 8), 0, ctx->stream>>>(W[i].p, in, H, norm[i].p);       // :511-513

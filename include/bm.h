@@ -207,6 +207,21 @@ typedef struct bm_dbm_cfg {
      * hidden layers, a context with a communicator; BM_EINVAL: a malformed ladder, sample_v == 0 or any sample_h == 0. */
     int32_t n_temps;
     const double* betas;
+    /* Classification DBM (DESIGN.md §5.7; no counterpart in the reference).  0: off.  n_classes = C >= 2 adds a one-of-C label
+     * y above the top hidden layer h_L: energy = the DBM's - e_y'U h_L - yb'e_y with U [C, H_L], yb [C].  Inside the engine y
+     * is hidden layer L + 1, multinomial with n_samples 1 and weight W_{L+1} = U^T.  Labels take values in {-1, 0, .., C-1};
+     * -1 marks an unlabelled row.  Training (bm_dbm_train_step_labeled): the mean-field E-step holds a labelled row's label
+     * at its one-hot e_t (never updated) and updates an unlabelled row's like any multinomial layer; the particles sweep v,
+     * h_1 .. h_L, y, drawing y (one categorical draw at site 16 + L); U takes l2, momentum and max-norm like any W, yb the
+     * plain momentum update from sum q(y) / rows - sum y / n_particles, with no sparsity term (sparsity_target / _cost keep
+     * their n_layers entries).  A batch labelled -1 throughout equals the plain DBM with a multinomial top layer of C units,
+     * n_samples 1, sampled, sparsity cost 0, bit for bit where that DBM runs (C > n_layers).  Queries run with y free:
+     * bm_dbm_predict_proba gives softmax(yb + mu_L U^T) from the E-step's final mu_L (a mean-field approximation of
+     * p(y|x)), bm_dbm_transform mu_L; bm_dbm_log_proba and AIS are refused (BM_EUNSUPPORTED).  Variables: the DBM's names for
+     * layers 0..L-1, plus "U", "dU" [C, H_L], "yb", "dyb" [C], the label particles "y" [n_particles, C] and the E-step's label
+     * slot "mu_y" [batch_size, C].  BM_EINVAL: n_classes < 0 or == 1, more than 7 hidden layers; BM_EUNSUPPORTED (the option
+     * named): float64, BM_COMPUTE_FP32, n_temps > 1, a context with a communicator. */
+    int32_t n_classes;
 } bm_dbm_cfg;
 
 int  bm_dbm_create(bm_ctx* ctx, const bm_dbm_cfg* cfg, bm_dbm** out);      /* DBM._make_tf_model, dbm.py:761-769 */
@@ -223,6 +238,14 @@ int  bm_dbm_init_particles(bm_dbm* dbm, uint64_t seed);
  * want_metrics != 0: out2 = {msre, n_mf_updates} (dbm.py:798-803) */
 int  bm_dbm_train_step(bm_dbm* dbm, const void* X, int32_t rows, double lr, double momentum, int32_t n_gibbs_steps,
                        uint64_t seed, uint32_t tick, int32_t want_metrics, double* out2);
+/* classification DBM (bm_dbm_cfg.n_classes >= 2): one training step with labels [rows] in [-1, n_classes) (BM_EINVAL before
+ * any launch otherwise; -1: unlabelled row); out2 as bm_dbm_train_step.  bm_dbm_train_step on a classification DBM is this
+ * call with every label -1.  BM_EINVAL on a DBM without a label layer. */
+int  bm_dbm_train_step_labeled(bm_dbm* dbm, const void* X, const int32_t* labels, int32_t rows, double lr, double momentum,
+                               int32_t n_gibbs_steps, uint64_t seed, uint32_t tick, int32_t want_metrics, double* out2);
+/* classification DBM: q(y|x) = softmax(yb + mu_L U^T) [rows, n_classes] (float32) after the E-step with y free, in chunks
+ * of batch_size rows; changes "mu..." like bm_dbm_transform.  BM_EINVAL on a DBM without a label layer. */
+int  bm_dbm_predict_proba(bm_dbm* dbm, const void* X, int32_t rows, float* out);
 /* validation msre / n_mf_updates; like the reference it also advances the persistent chains (dbm.py:523, 810-816) */
 int  bm_dbm_val_metrics(bm_dbm* dbm, const void* X, int32_t rows, int32_t n_gibbs_steps, uint64_t seed, uint32_t tick, double* out2);
 int  bm_dbm_transform(bm_dbm* dbm, const void* X, int32_t rows, void* out);       /* mu of the last layer, dbm.py:526-528,859-872 */
