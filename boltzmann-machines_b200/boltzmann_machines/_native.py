@@ -72,6 +72,8 @@ class DbmCfg(C.Structure):
         ('n_temps', C.c_int32),
         ('betas', C.POINTER(C.c_double)),
         ('n_classes', C.c_int32),
+        ('centering', C.c_int32),
+        ('offset_rate', C.c_double),
     ]
 
 
@@ -803,11 +805,19 @@ class CudaDBM(object):
         if self.C:
             self.compute = cfg.get('compute') or 'bf16'
             c.compute = COMPUTE[self.compute]
+        # centering: data-mean offsets and offset-centred gradients (tensor-core engine only, which it asks for unless the
+        # caller names a compute mode); the variables v_offset, h_offset..., offsets_set
+        self.centering = bool(cfg.get('centering', False))
+        if self.centering:
+            c.centering = 1
+            c.offset_rate = float(cfg.get('offset_rate', 0.01))
+            self.compute = cfg.get('compute') or 'bf16'
+            c.compute = COMPUTE[self.compute]
         h = C.c_void_p()
         rc = self._lib.bm_dbm_create(self.ctx.handle, C.byref(c), C.byref(h))
         if rc in (-1, -5):
             err = self._lib.bm_last_error().decode('utf-8', 'replace')
-            if err.startswith('parallel tempering') or err.startswith('classification DBM'):
+            if err.startswith('parallel tempering') or err.startswith('classification DBM') or err.startswith('centering'):
                 raise (NotImplementedError if rc == -5 else ValueError)('libbm: ' + err)
         check(rc)
         self.handle = h
@@ -822,6 +832,10 @@ class CudaDBM(object):
             self._shapes['v_pt'] = (self.T - 1, self.M, self.V)
             for i in range(self.L):
                 self._shapes['h_pt' + _sfx(i)] = (self.T - 1, self.M, self.Hs[i])
+        if self.centering:
+            self._shapes.update({'v_offset': (self.V,), 'offsets_set': (1,)})
+            for i in range(self.L):
+                self._shapes['h_offset' + _sfx(i)] = (self.Hs[i],)
         if self.C:
             Cn, H = self.C, self.Hs[-1]
             self._shapes.update({'U': (Cn, H), 'dU': (Cn, H), 'yb': (Cn,), 'dyb': (Cn,), 'y': (self.M, Cn),

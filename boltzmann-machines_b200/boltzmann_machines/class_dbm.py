@@ -49,6 +49,8 @@ class ClassificationDBM(DBM):
     def __init__(self, rbms=None, pt_betas=None, model_path='class_dbm_model/', *args, **kwargs):
         if pt_betas is not None:
             raise NotImplementedError('ClassificationDBM does not support parallel tempering (pt_betas)')
+        if kwargs.get('centering'):
+            raise NotImplementedError('ClassificationDBM does not support centering')
         self.n_classes_ = None
         super(ClassificationDBM, self).__init__(rbms=rbms, pt_betas=None, model_path=model_path, *args, **kwargs)
         if np.dtype(self.dtype) != np.float32:

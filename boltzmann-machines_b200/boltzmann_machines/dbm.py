@@ -51,6 +51,12 @@ class DBM(EnergyBasedModel):
         slots.  The gradient, ``sample_v`` and the particles ``v`` / ``h...`` are slot 0's.  Needs the tensor-core engine
         (float32, Bernoulli units) and sampled states in every layer; ``pt_swap_rates_`` holds the last epoch's
         acceptance rate of each pair (m, m+1) (None for a pair the epoch did not propose).
+    centering : False (default), or True to train the centered DBM (not in the reference; Montavon & Mueller, *Deep
+        Boltzmann machines and the centering trick*, 2012): every layer's states are taken relative to an offset, the data
+        mean of the layer, which conditions the gradient so that a DBM can be trained from scratch.  The model's
+        distribution and every query are those of the stored (W, b); only the training step changes.  The offsets (scope
+        ``offsets``) are set from the first batch and then follow an exponential moving average of the batch means with
+        rate ``offset_rate`` in [0, 1].  Needs the tensor-core engine (float32); not for ``ClassificationDBM``.
     """
     _MUTABLE_PREFIXES = ('mu', 'v', 'h')
 
@@ -64,7 +70,7 @@ class DBM(EnergyBasedModel):
                  train_metrics_every_iter=10, val_metrics_every_epoch=1,
                  verbose=False, save_after_each_epoch=True,
                  display_filters=0, display_particles=0, v_shape=(28, 28),
-                 model_path='dbm_model/', pt_betas=None, *args, **kwargs):
+                 model_path='dbm_model/', pt_betas=None, centering=False, offset_rate=0.01, *args, **kwargs):
         super(DBM, self).__init__(model_path=model_path, *args, **kwargs)
         self.n_layers_ = len(rbms) if rbms is not None else None
         self.n_visible_ = None
@@ -117,6 +123,10 @@ class DBM(EnergyBasedModel):
         self._check_pt()
         self.pt_swap_rates_ = None
 
+        self.centering = bool(centering)
+        self.offset_rate = float(offset_rate)
+        self._check_centering()
+
         self.epoch_ = 0
         self.iter_ = 0
         self.n_samples_generated_ = 0
@@ -137,6 +147,15 @@ class DBM(EnergyBasedModel):
                 raise NotImplementedError('parallel tempering is not supported with gaussian visibles')
             if any(h['kind'] != 'bernoulli' for h in self.layers_['h']):
                 raise NotImplementedError('parallel tempering is not supported with multinomial hidden layers')
+
+    def _check_centering(self):
+        """The refusals of the engine (include/bm.h, bm_dbm_cfg.centering) as far as the constructor can tell."""
+        if not (0.0 <= self.offset_rate <= 1.0):
+            raise ValueError('offset_rate must lie in [0, 1], got {0}'.format(self.offset_rate))
+        if not self.centering:
+            return
+        if np.dtype(self.dtype) != np.float32:
+            raise NotImplementedError('centering runs on the tensor-core engine: float32 models only')
 
     # ---- composition from pre-trained RBMs (dbm.py:207-231, 266-291) ---------------------
     def load_rbms(self, rbms):
@@ -191,6 +210,7 @@ class DBM(EnergyBasedModel):
             'variational_params': per('mu'),
             'hidden_means_accumulators': per('q_means') + per('mu_means'),
             'negative_particles': ('v',) + per('h') + tempered,
+            'offsets': ('v_offset',) + per('h_offset') + ('offsets_set',) if self.centering else (),
         }
 
     def _tf_name(self, scope, name):
@@ -219,6 +239,9 @@ class DBM(EnergyBasedModel):
         )
         if self.pt_betas is not None:
             cfg['pt_betas'] = list(self.pt_betas)
+        if self.centering:
+            cfg['centering'] = True
+            cfg['offset_rate'] = self.offset_rate
         if 'sigma' in lay['v']:
             cfg['sigma'] = np.broadcast_to(np.asarray(lay['v']['sigma'], dtype=np.float64), (self.n_visible_,)).copy()
         return cfg

@@ -708,6 +708,17 @@ struct Dbm : DbmBase {
 
 using namespace bm;
 
+// Centering (bm_dbm_cfg.centering / offset_rate): what is refused before anything is allocated.  0 is off.
+static void check_centering_cfg(const Ctx* ctx, const bm_dbm_cfg& f) {
+    if (f.centering == 0) return;
+    BM_REQUIRE(std::isfinite(f.offset_rate) && f.offset_rate >= 0.0 && f.offset_rate <= 1.0, "centering: offset_rate must lie in [0, 1]");
+    if (f.n_classes != 0) throw Error(BM_EUNSUPPORTED, "centering is not supported for classification DBMs (n_classes)");
+    if (f.dtype != BM_DTYPE_F32 || f.compute != BM_COMPUTE_BF16)
+        throw Error(BM_EUNSUPPORTED, "centering runs on the tensor-core engine only (float32 models, compute bf16)");
+    if (!DbmTC::supports(f)) throw Error(BM_EUNSUPPORTED, "centering: the model does not run on the tensor-core engine");
+    if (ctx->nranks > 1) throw Error(BM_EUNSUPPORTED, "centering is not supported on a context with a communicator");
+}
+
 extern "C" {
 
 int bm_dbm_create(bm_ctx* hctx, const bm_dbm_cfg* cfg, bm_dbm** out) {
@@ -719,6 +730,7 @@ int bm_dbm_create(bm_ctx* hctx, const bm_dbm_cfg* cfg, bm_dbm** out) {
     BM_REQUIRE(cfg->n_particles > 0 && cfg->batch_size > 0, "n_particles and batch_size must be positive");
     BM_REQUIRE(cfg->v_kind != BM_UNIT_GAUSSIAN || cfg->sigma, "gaussian visible layer needs sigma");
     BM_REQUIRE(cfg->n_classes >= 0 && cfg->n_classes != 1, "classification DBM: n_classes must be 0 (no label layer) or at least 2");
+    check_centering_cfg(ctx, *cfg);
     if (cfg->n_classes >= 2) ClassDbmTC::check_cfg(ctx, *cfg);      // then n_temps <= 1: at most [1.0], no tempering
     check_pt_cfg(ctx, *cfg);
     if (cfg->n_temps >= 1 && !DbmTC::supports(*cfg)) throw Error(BM_EUNSUPPORTED, "parallel tempering: the model does not run on the tensor-core engine");

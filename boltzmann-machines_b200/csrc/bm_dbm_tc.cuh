@@ -181,6 +181,103 @@ __global__ void dbm_grad_combine_kernel(const float* __restrict__ pos, int sp, c
     }
 }
 
+// ---- centering (DESIGN.md §5.8) ---------------------------------------------------------------------------------------------
+// Unit layers j = 0..L (0 = visible): offsets o_j, data side d_j (X, mu_{j-1}) and particle side p_j (v, h_{j-1}).  Every fp32
+// operation below is written out with _rn intrinsics so that nothing is contracted and the host restatements follow it exactly.
+struct CenterArgs {
+    int n_layers;                   // L + 1
+    int n[9];
+    const float* dsum[9];           // column sums of d_j over the rows present
+    const float* psum[9];           // column sums of p_j over the particles
+    float* o[9];                    // the offsets of this step (written on a model's first step)
+    float* o_next[9];               // the offsets after this step: (1 - rate) o + rate mean_rows(d)
+    float* s[9];                    // s_j = dsum / N - psum / M
+    float rows, inv_n, inv_m, keep, rate;
+    int init;                       // a model's first step: o_j <- mean_rows(d_j) first
+};
+__global__ void dbm_center_stats_kernel(CenterArgs a) {
+    const int j = blockIdx.y, u = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= a.n_layers || u >= a.n[j]) return;
+    const float d = a.dsum[j][u], mean = __fdiv_rn(d, a.rows);
+    float o = a.o[j][u];
+    if (a.init) { o = mean; a.o[j][u] = o; }
+    a.s[j][u] = __fsub_rn(__fmul_rn(d, a.inv_n), __fmul_rn(a.psum[j][u], a.inv_m));
+    a.o_next[j][u] = __fadd_rn(__fmul_rn(a.keep, o), __fmul_rn(a.rate, mean));
+}
+
+// The centered gradient of W_i (H = n_{i+1} columns) from the split-K slices of the plain one:
+//   G^c = (pos / N - neg / M) - o_i s_{i+1}' - s_i o_{i+1}' + corr o_i o_{i+1}',   corr = rows / N - 1
+// the literal restatement of sum (d_i - o_i)(d_{i+1} - o_{i+1})' / N - sum (p_i - o_i)(p_{i+1} - o_{i+1})' / M.  The first term
+// is dbm_grad_combine_kernel's expression, so zero offsets give its result bit for bit.
+__global__ void dbm_centered_grad_combine_kernel(const float* __restrict__ pos, int sp, const float* __restrict__ neg, int sn,
+                                                 size_t stride, float inv_n, float inv_m, int H,
+                                                 const float* __restrict__ o_in, const float* __restrict__ s_in,
+                                                 const float* __restrict__ o_out, const float* __restrict__ s_out, float corr,
+                                                 float* __restrict__ G, size_t n) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        float a = 0.f, b = 0.f;
+        for (int s = 0; s < sp; ++s) a += pos[(size_t)s * stride + i];
+        for (int s = 0; s < sn; ++s) b += neg[(size_t)s * stride + i];
+        const size_t r = i / (size_t)H, c = i % (size_t)H;
+        float g = a * inv_n - b * inv_m;
+        g = __fsub_rn(g, __fmul_rn(o_in[r], s_out[c]));
+        g = __fsub_rn(g, __fmul_rn(s_in[r], o_out[c]));
+        g = __fadd_rn(g, __fmul_rn(corr, __fmul_rn(o_in[r], o_out[c])));
+        G[i] = g;
+    }
+}
+
+// The coupling of unit layer j to the offsets of its neighbours, c_j = W_{j-1}' o_{j-1} + W_j o_{j+1} (missing terms dropped),
+// in fp32.  mode 0: cpl_j <- c_j.  mode 1: b_j <- b_j - (c_j - cpl_j), which keeps a_j = b_j + c_j when W has changed.
+// Block (32, 8) per 32 units of layer blockIdx.y.  The column term: thread (x, y) sums rows y, y + 8, ... of column x with
+// fma, then the 8 partials add in order; the row term: warp y takes units y, y + 8, y + 16, y + 24, lane l sums k = l, l + 32,
+// ... with fma, then the xor tree; c = colterm + rowterm.
+struct CouplingArgs {
+    int n_layers;                   // L + 1
+    int n[9];
+    const float* W[8];              // W_i [n_i, n_{i+1}]
+    const float* o[9];
+    float* cpl[9];
+    float* b[9];                    // vb, hb, hb_1, ...
+    int mode;
+};
+__global__ void __launch_bounds__(256) dbm_coupling_kernel(CouplingArgs a) {
+    __shared__ float colp[8][33];
+    __shared__ float rowp[32];
+    const int j = blockIdx.y, tx = threadIdx.x, ty = threadIdx.y;
+    const int n = a.n[j], u0 = blockIdx.x * 32;
+    if (u0 >= n) return;                                     // uniform over the block
+    float cp = 0.f;
+    if (j > 0 && u0 + tx < n) {
+        const float* W = a.W[j - 1];
+        const float* o = a.o[j - 1];
+        for (int r = ty; r < a.n[j - 1]; r += 8) cp = __fmaf_rn(W[(size_t)r * n + u0 + tx], o[r], cp);
+    }
+    colp[ty][tx] = cp;
+    for (int q = ty; q < 32; q += 8) {
+        float s = 0.f;
+        if (j + 1 < a.n_layers && u0 + q < n) {
+            const int m = a.n[j + 1];
+            const float* W = a.W[j] + (size_t)(u0 + q) * m;
+            const float* o = a.o[j + 1];
+            for (int k = tx; k < m; k += 32) s = __fmaf_rn(W[k], o[k], s);
+        }
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, off));
+        if (tx == 0) rowp[q] = s;
+    }
+    __syncthreads();
+    if (ty == 0 && u0 + tx < n) {
+        float c = 0.f;
+#pragma unroll
+        for (int y = 0; y < 8; ++y) c = __fadd_rn(c, colp[y][tx]);
+        c = __fadd_rn(c, rowp[tx]);
+        const int u = u0 + tx;
+        if (a.mode == 0) a.cpl[j][u] = c;
+        else a.b[j][u] = __fsub_rn(a.b[j][u], __fsub_rn(c, a.cpl[j][u]));
+    }
+}
+
 // AIS unit update from fp32 pre-activations: out = sample ? (u < sigmoid(beta * pre)) : sigmoid(beta * pre), bf16.
 // pre == nullptr: pre-activation 0 (the uniform base-rate draw x_0 ~ Ber(1/2), dbm.py:700-702).
 // ldo % 4 == 0 (buffers are padded to 64 columns): the four columns of a Philox block leave as one 8-byte store.
@@ -400,6 +497,14 @@ struct DbmTC : Dbm<float> {
     std::vector<long long> pt_proposed;          // [T - 1] swaps proposed since create (known on the host)
     std::vector<DevBuf<float>> pt_pre;           // per layer [T M, H_i]: h_{i-1} W_i + c_i of the current particles
     std::map<std::tuple<int, int, int>, TcChain> pt_progs;   // committed tempered sweeps: keyed by (sweeps, sampled, t0)
+    // centering (bm_dbm_cfg.centering, DESIGN.md §5.8): per unit layer j = 0..L the offsets off[oc][j] (a step's moved offsets
+    // go to off[1 - oc], which then becomes current), s_j of the step and the coupling c_j before the update.  Off: none of it
+    // exists and the step is the plain one, launch for launch.
+    bool centering = false;
+    float offset_rate = 0.f;
+    bool offsets_set = false;                    // "offsets_set": the first step sets the offsets to the data means
+    int oc = 0;
+    std::vector<DevBuf<float>> off[2], cen_s, cpl;
 
     // float32; Bernoulli or Gaussian visibles; Bernoulli and multinomial hidden layers in any order (the DBM's multinomial
     // particles are refused on a sharded context by init_particles)
@@ -446,6 +551,13 @@ struct DbmTC : Dbm<float> {
         int hmax = 0;
         for (int i = 0; i < L; ++i) if (multinomial(i)) hmax = std::max(hmax, Hs[i]);
         if (hmax) pre_f32.ensure((size_t)std::max(B, M) * hmax);
+        if (f.centering) {                       // validated by bm_dbm_create (check_centering_cfg)
+            centering = true;
+            offset_rate = (float)f.offset_rate;
+            for (auto* v : {&off[0], &off[1], &cen_s, &cpl}) v->resize(L + 1);
+            for (int j = 0; j <= L; ++j)
+                for (DevBuf<float>* b : {&off[0][j], &off[1][j], &cen_s[j], &cpl[j]}) { b->ensure(size_of(j, V, Hs)); b->zero(ctx->stream); }
+        }
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
     }
 
@@ -511,7 +623,26 @@ struct DbmTC : Dbm<float> {
         }
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
     }
+    // centering's variables: "v_offset" [V], "h_offset", "h_offset_<i>" [H_i] and "offsets_set" [1] (0 or 1).  false: not one.
+    bool offset_param(const std::string& name, void* host, const void* in, size_t bytes) {
+        if (!centering) return false;
+        if (name == "offsets_set") {
+            BM_REQUIRE(bytes == sizeof(float), "size mismatch for 'offsets_set'");
+            float f = offsets_set ? 1.f : 0.f;
+            if (in) { memcpy(&f, in, sizeof(f)); offsets_set = f != 0.f; } else memcpy(host, &f, sizeof(f));
+            return true;
+        }
+        int j = name == "v_offset" ? 0 : -1;
+        for (int i = 0; i < L && j < 0; ++i) if (name == "h_offset" + sfx(i)) j = i + 1;
+        if (j < 0) return false;
+        BM_REQUIRE(bytes == (size_t)size_of(j, V, Hs) * sizeof(float), "size mismatch for '" + name + "'");
+        if (in) BM_CUDA(cudaMemcpyAsync(off[oc][j].p, in, bytes, cudaMemcpyHostToDevice, ctx->stream));
+        else BM_CUDA(cudaMemcpyAsync(host, off[oc][j].p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        BM_CUDA(cudaStreamSynchronize(ctx->stream));
+        return true;
+    }
     void set_param(const char* name, const void* host, size_t bytes) override {
+        if (offset_param(name, nullptr, host, bytes)) return;
         const int pt = pt_layer(name);
         if (pt >= 0) { pt_param(pt, nullptr, host, bytes); return; }
         widen_particles();                         // the fp32 copies become the truth for one moment
@@ -520,6 +651,7 @@ struct DbmTC : Dbm<float> {
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
     }
     void get_param(const char* name, void* host, size_t bytes) override {
+        if (offset_param(name, host, nullptr, bytes)) return;
         const int pt = pt_layer(name);
         if (pt >= 0) { pt_param(pt, host, nullptr, bytes); return; }
         widen_particles();
@@ -970,8 +1102,48 @@ struct DbmTC : Dbm<float> {
         };
         half(pos, mu_b[i].p, pos_rows, sp, Gp[i].p);
         half(neg, h_b[i].p, M, sn, Gp[i].p + (size_t)sp * stride);
-        dbm_grad_combine_kernel<<<592, 256, 0, ctx->stream>>>(Gp[i].p, sp, Gp[i].p + (size_t)sp * stride, sn, stride,
-                                                              1.0f / n_div, 1.0f / m_div, G[i].p, stride);
+        if (centering)
+            dbm_centered_grad_combine_kernel<<<592, 256, 0, ctx->stream>>>(
+                Gp[i].p, sp, Gp[i].p + (size_t)sp * stride, sn, stride, 1.0f / n_div, 1.0f / m_div, H, off[oc][i].p, cen_s[i].p,
+                off[oc][i + 1].p, cen_s[i + 1].p, (float)((double)pos_rows / (double)n_div - 1.0), G[i].p, stride);
+        else
+            dbm_grad_combine_kernel<<<592, 256, 0, ctx->stream>>>(Gp[i].p, sp, Gp[i].p + (size_t)sp * stride, sn, stride,
+                                                                  1.0f / n_div, 1.0f / m_div, G[i].p, stride);
+        count_launch(ctx);
+    }
+
+    // centering: s_j and (first step) the offsets from the step's column sums, the moved offsets into off[1 - oc]
+    void center_stats(int rows, float N, float Mp) {
+        CenterArgs a;
+        memset(&a, 0, sizeof(a));
+        a.n_layers = L + 1;
+        int nmax = 0;
+        for (int j = 0; j <= L; ++j) {
+            a.n[j] = size_of(j, V, Hs); nmax = std::max(nmax, a.n[j]);
+            a.dsum[j] = j == 0 ? xsum.p : musum[j - 1].p;
+            a.psum[j] = j == 0 ? vsum.p : hsum[j - 1].p;
+            a.o[j] = off[oc][j].p; a.o_next[j] = off[1 - oc][j].p; a.s[j] = cen_s[j].p;
+        }
+        a.rows = (float)rows; a.inv_n = 1.0f / N; a.inv_m = 1.0f / Mp;
+        a.keep = (float)(1.0 - (double)offset_rate); a.rate = offset_rate;
+        a.init = offsets_set ? 0 : 1;
+        dbm_center_stats_kernel<<<dim3((nmax + 255) / 256, L + 1), 256, 0, ctx->stream>>>(a);
+        count_launch(ctx);
+        offsets_set = true;
+    }
+    // centering: mode 0 stores c_j of the current W and offsets; mode 1 takes the change of c_j out of b_j
+    void coupling(int mode) {
+        CouplingArgs a;
+        memset(&a, 0, sizeof(a));
+        a.n_layers = L + 1;
+        int nmax = 0;
+        for (int j = 0; j <= L; ++j) {
+            a.n[j] = size_of(j, V, Hs); nmax = std::max(nmax, a.n[j]);
+            if (j < L) a.W[j] = W[j].p;
+            a.o[j] = off[oc][j].p; a.cpl[j] = cpl[j].p; a.b[j] = j == 0 ? vb.p : hb[j - 1].p;
+        }
+        a.mode = mode;
+        dbm_coupling_kernel<<<dim3((nmax + 31) / 32, L + 1), dim3(32, 8), 0, ctx->stream>>>(a);
         count_launch(ctx);
     }
 
@@ -984,8 +1156,9 @@ struct DbmTC : Dbm<float> {
         const int nr = nranks();                               // data parallelism: see the header of bm_dbm.cu
         const float N = (float)((double)B * nr), Mp = (float)((double)M * nr);      // configured (global) sizes (dbm.py:254-255)
         const float rows_g = (float)((double)rows * nr);
-        for (int i = 0; i < L; ++i) gradient_tc(i, i == 0 ? Xb.p : mu_b[i - 1].p, rows, i == 0 ? v_b.p : h_b[i - 1].p, N, Mp);
-        {   // column sums of mu_i (over the batch rows) and of h_i, v (over the particles), three per pair of launches
+        // column sums of mu_i (over the batch rows) and of h_i, v (over the particles), three per pair of launches; X over the rows.
+        // A centered step reads them in its gradients' combine, so they go first there.
+        auto column_sums = [&]() {
             std::vector<const bf16_t*> P; std::vector<int> ld, nc; std::vector<float*> out;
             auto flush = [&](int nrows) {
                 for (size_t o = 0; o < P.size(); o += 3) {
@@ -999,8 +1172,15 @@ struct DbmTC : Dbm<float> {
             for (int i = 0; i < L; ++i) { P.push_back(h_b[i].p); ld.push_back(ldn[i + 1]); nc.push_back(Hs[i]); out.push_back(hsum[i].p); }
             P.push_back(v_b.p); ld.push_back(ldn[0]); nc.push_back(V); out.push_back(vsum.p);
             flush(M);
+            launch_colsum<float>(ctx, X, V, (const float*)nullptr, 0, rows, V, 1.f, 0.f, xsum.p);
+        };
+        if (centering) {
+            column_sums();
+            center_stats(rows, N, Mp);
+            coupling(0);
         }
-        launch_colsum<float>(ctx, X, V, (const float*)nullptr, 0, rows, V, 1.f, 0.f, xsum.p);
+        for (int i = 0; i < L; ++i) gradient_tc(i, i == 0 ? Xb.p : mu_b[i - 1].p, rows, i == 0 ? v_b.p : h_b[i - 1].p, N, Mp);
+        if (!centering) column_sums();
         allreduce_step_statistics();
         dbm_vbias_kernel<float><<<(V + 255) / 256, 256, 0, ctx->stream>>>(V, xsum.p, vsum.p, rows_g, Mp, vb.p, dvb.p, (float)lr, (float)mom);
         count_launch(ctx);
@@ -1022,6 +1202,10 @@ struct DbmTC : Dbm<float> {
             max_norm_scale_kernel<float><<<dim3((H + 255) / 256, in < 32768 ? in : 32768), 256, 0, ctx->stream>>>(W[i].p, in, H, norm[i].p, (float)max_norm);
             count_launch(ctx);
             refresh_shadow(i);
+        }
+        if (centering) {          // b_j = a_j - c_j with the new W and the step's offsets; then the moved offsets
+            coupling(1);
+            oc = 1 - oc;
         }
     }
 

@@ -222,6 +222,19 @@ typedef struct bm_dbm_cfg {
      * slot "mu_y" [batch_size, C].  BM_EINVAL: n_classes < 0 or == 1, more than 7 hidden layers; BM_EUNSUPPORTED (the option
      * named): float64, BM_COMPUTE_FP32, n_temps > 1, a context with a communicator. */
     int32_t n_classes;
+    /* Centering (Montavon & Mueller 2012; DESIGN.md §5.8; not in the reference).  0: off.  centering != 0 trains the
+     * centered DBM E_c(x) = -sum_i (x_i - o_i)'W_i (x_{i+1} - o_{i+1}) - sum_j (x_j - o_j)'a_j with data-mean offsets o_j.
+     * The engine keeps storing the plain parameters (W, b) with b_j = a_j - W_{j-1}'o_{j-1} - W_j o_{j+1}, so every
+     * query, particle sweep, swap and AIS reads what it reads without centering.  A training step takes the centered
+     * gradient G_i - o_i s_{i+1}' - s_i o_{i+1}' + (rows / batch_size - 1) o_i o_{i+1}' (s_j = sum data_j / batch_size -
+     * sum particles_j / n_particles), applies l2, sparsity, momentum and max-norm to it and to the a_j where they apply to
+     * G and b, re-derives b from the new W, then moves o_j <- (1 - offset_rate) o_j + offset_rate mean_rows(data_j).  The
+     * first step of a model sets o_j to the batch's data means.  Variables: "v_offset" [V], "h_offset", "h_offset_1"...
+     * [H_i] and "offsets_set" [1] (0 until the first step; 1 afterwards).  BM_EINVAL: offset_rate outside [0, 1];
+     * BM_EUNSUPPORTED (the option named): float64, BM_COMPUTE_FP32 or any model DbmTC does not run, n_classes > 0, a
+     * context with a communicator. */
+    int32_t centering;
+    double offset_rate;
 } bm_dbm_cfg;
 
 int  bm_dbm_create(bm_ctx* ctx, const bm_dbm_cfg* cfg, bm_dbm** out);      /* DBM._make_tf_model, dbm.py:761-769 */
