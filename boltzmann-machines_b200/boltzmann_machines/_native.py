@@ -33,7 +33,7 @@ EXPORTS = (
     'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows', 'bm_dbm_pt_counts', 'bm_debug_dbm_multinomial_rows',
     'bm_dbm_train_step_labeled', 'bm_dbm_predict_proba',
     'bm_crbm_create', 'bm_crbm_destroy', 'bm_crbm_set_param', 'bm_crbm_get_param', 'bm_crbm_init_weights',
-    'bm_crbm_train_step', 'bm_crbm_predict_proba', 'bm_crbm_transform',
+    'bm_crbm_train_step', 'bm_crbm_predict_proba', 'bm_crbm_transform', 'bm_crbm_debug_last_step',
     'bm_rbm_group_create', 'bm_rbm_group_destroy', 'bm_rbm_group_train_epoch', 'bm_rbm_group_train_epoch_u8',
     'bm_rbm_group_train_epoch_bf16',
 )
@@ -174,6 +174,7 @@ def load_library(path=None):
         'bm_crbm_init_weights': [vp, dbl, u64, u64],
         'bm_crbm_train_step': [vp, vp, vp, i32, dbl, dbl, i32, u64, u32, i32, C.POINTER(dbl)],
         'bm_crbm_predict_proba': [vp, vp, i32, vp], 'bm_crbm_transform': [vp, vp, i32, vp],
+        'bm_crbm_debug_last_step': [vp, C.c_char_p, vp, sz],
         'bm_rbm_group_create': [vp, vp, i32, C.POINTER(vp)],
     }
     group_epoch = [vp, vp, i64, i32, vp, vp, i32, vp, vp, vp, vp, vp, vp]
@@ -1012,7 +1013,23 @@ class CudaCRBM(object):
             raise ValueError('{0} labels for {1} rows'.format(y.shape[0], X.shape[0]))
         check(self._lib.bm_crbm_train_step(self.handle, X.ctypes.data, y.ctypes.data, X.shape[0], float(lr), float(momentum),
                                            int(k), int(seed) & (2 ** 64 - 1), int(tick), 1 if metrics else 0, self._out2))
+        self._last_rows = X.shape[0]
         return {'nll': float(self._out2[0]), 'accuracy': float(self._out2[1])} if metrics else None
+
+    DEBUG_WIDTHS = {'A': 'H', 'P': 'C', 'y0': None, 'G': 'H', 'h0': 'H', 'x_k': 'V', 'y_k': 'C', 'h_k': 'H', 'aH': 'H'}
+
+    def debug_last_step(self, names=('A', 'P', 'y0', 'G')):
+        """the last train_step's buffers (bm_crbm_debug_last_step): A and P float32, y0 int32, the bf16 ones widened to
+        float32.  The chain's 'h0', 'x_k', 'y_k', 'h_k', 'aH' exist only when the chain ran ('h0' only at k = 1)."""
+        rows = getattr(self, '_last_rows', 0)
+        out = {}
+        for n in names:
+            w = self.DEBUG_WIDTHS[n]
+            shape = (rows,) if w is None else (rows, getattr(self, w))
+            a = np.empty(shape, dtype={'A': np.float32, 'P': np.float32, 'y0': np.int32}.get(n, np.uint16))
+            check(self._lib.bm_crbm_debug_last_step(self.handle, n.encode(), a.ctypes.data, a.nbytes))
+            out[n] = (a.astype(np.uint32) << 16).view(np.float32) if a.dtype == np.uint16 else a
+        return out
 
     def predict_proba(self, X):
         X = self._batch(X)

@@ -357,6 +357,11 @@ struct ClassRbmTC : DbmTC {
     DevBuf<double> nll;
     DevBuf<int> correct, lab, y0;
     DevBuf<bf16_t> Gb, aHb;
+    // what the last hybrid_step left for debug_last_step: its rows (0: none since the last predict), chain length, whether
+    // the chain ran, and the buffer holding its last sweep's h
+    int last_rows = 0, last_k = 0;
+    bool last_gen = false;
+    const bf16_t* last_hk = nullptr;
 
     // refusals name the option (BM_EUNSUPPORTED); shapes and classes are BM_EINVAL
     static void check_cfg(Ctx* ctx, const bm_crbm_cfg& f) {
@@ -472,6 +477,7 @@ struct ClassRbmTC : DbmTC {
         const bool gen = alpha > 0.f || semi;                    // the chain runs for the generative terms of either kind
         BM_REQUIRE(!gen || k >= 1, "n_gibbs_steps must be at least 1 when alpha > 0 or a row is unlabelled");
         BM_REQUIRE(!want || out, "metrics requested without a buffer");
+        last_rows = 0;
         upload_tc(Xh, rows);
         BM_CUDA(cudaMemcpyAsync(lab.p, labels, (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
         forward(rows);
@@ -519,6 +525,7 @@ struct ClassRbmTC : DbmTC {
                                                                                  lab.p, beta, uyh, hku, xdu, yku);
             count_launch(ctx);
         }
+        last_rows = rows; last_k = k; last_gen = gen; last_hk = hc;
         {   // X^T G [- X_k^T (alpha H_k)]: one split-K op over the batch rows
             TcGemm g;
             g.M = V; g.N = H;
@@ -567,6 +574,7 @@ struct ClassRbmTC : DbmTC {
         BM_REQUIRE(rows >= 1, "empty batch");
         const float* X = static_cast<const float*>(Xh);
         const int w = hidden ? H : C;
+        last_rows = 0;                                         // A and P no longer hold the last step's values
         for (int r0 = 0; r0 < rows; r0 += B) {
             const int n = std::min(B, rows - r0);
             upload_tc(X + (size_t)r0 * V, n);
@@ -576,6 +584,33 @@ struct ClassRbmTC : DbmTC {
             BM_CUDA(cudaMemcpyAsync(out + (size_t)r0 * w, hidden ? Sh.p : P.p, (size_t)n * w * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
             BM_CUDA(cudaStreamSynchronize(ctx->stream));
         }
+    }
+
+    // copies one of the last hybrid_step's buffers to the host, [rows, width] without padding: device to host only, no launch
+    void debug_last_step(const std::string& n, void* host, size_t bytes) {
+        BM_REQUIRE(last_rows > 0, "no training step since the engine was created or last predicted");
+        const int rows = last_rows;
+        auto copy = [&](const void* src, int width, size_t ld, size_t elem) {
+            BM_REQUIRE(bytes == (size_t)rows * width * elem, "size mismatch for '" + n + "'");
+            BM_CUDA(cudaMemcpy2DAsync(host, (size_t)width * elem, src, ld * elem, (size_t)width * elem, rows, cudaMemcpyDeviceToHost,
+                                      ctx->stream));
+            BM_CUDA(cudaStreamSynchronize(ctx->stream));
+        };
+        const bool chain = n == "h0" || n == "x_k" || n == "y_k" || n == "h_k" || n == "aH";
+        if (chain) BM_REQUIRE(last_gen, "'" + n + "' is written only by a step whose chain ran (alpha > 0 or an unlabelled row)");
+        if (n == "A") copy(A.p, H, H, sizeof(float));
+        else if (n == "P") copy(P.p, C, C, sizeof(float));
+        else if (n == "y0") copy(y0.p, 1, 1, sizeof(int));
+        else if (n == "G") copy(Gb.p, H, ldn[1], sizeof(bf16_t));
+        else if (n == "h0") {
+            BM_REQUIRE(last_k == 1, "'h0' survives only a step with n_gibbs_steps = 1 (later sweeps overwrite it)");
+            copy(h_b[0].p, H, ldn[1], sizeof(bf16_t));
+        }
+        else if (n == "x_k") copy(v_b.p, V, ldn[0], sizeof(bf16_t));
+        else if (n == "y_k") copy(h_b[1].p, C, ldn[2], sizeof(bf16_t));
+        else if (n == "h_k") copy(last_hk, H, ldn[1], sizeof(bf16_t));
+        else if (n == "aH") copy(aHb.p, H, ldn[1], sizeof(bf16_t));
+        else throw Error(BM_EINVAL, "unknown step buffer '" + n + "'");
     }
 };
 
@@ -619,6 +654,9 @@ int bm_crbm_train_step(bm_crbm* h, const void* X, const int32_t* labels, int32_t
     BM_API_BEGIN CRBM_ENTER(h) BM_REQUIRE(X && labels, "null argument");
     CRBM(h)->hybrid_step(X, labels, rows, lr, momentum, k, seed, tick, want_metrics, out2);
     BM_API_END
+}
+int bm_crbm_debug_last_step(bm_crbm* h, const char* name, void* host, size_t bytes) {
+    BM_API_BEGIN CRBM_ENTER(h) BM_REQUIRE(name && host, "null argument"); CRBM(h)->debug_last_step(name, host, bytes); BM_API_END
 }
 int bm_crbm_predict_proba(bm_crbm* h, const void* X, int32_t rows, float* out) {
     BM_API_BEGIN CRBM_ENTER(h) BM_REQUIRE(X && out, "null argument"); CRBM(h)->predict(X, rows, out, false); BM_API_END

@@ -382,6 +382,19 @@ int  bm_crbm_init_weights(bm_crbm* crbm, double stddev, uint64_t op_seed_w, uint
  * when the batch has none) */
 int  bm_crbm_train_step(bm_crbm* crbm, const void* X, const int32_t* labels, int32_t rows, double lr, double momentum,
                         int32_t n_gibbs_steps, uint64_t seed, uint32_t tick, int32_t want_metrics, double* out2);
+/* test hook: copies one buffer of the last bm_crbm_train_step to the host, [rows, width] row-major without padding, where rows
+ * is that step's batch.  Device-to-host copies only: it launches nothing and changes no state.  Names and widths:
+ *   "A"   float32 [rows, n_hidden]    X W (bf16 operands, fp32 accumulation, no bias)
+ *   "P"   float32 [rows, n_classes]   p(y|x)
+ *   "y0"  int32   [rows]              the chain's start label (meaningful for rows labelled -1 only)
+ *   "G"   uint16  [rows, n_hidden]    bf16 bits of (1 + alpha) S_t - S^ (beta S^ on unlabelled rows), the dW operand
+ * and, when the step's chain ran (alpha > 0 or an unlabelled row), bf16 bits of:
+ *   "h0"  [rows, n_hidden]            the chain's start (only after a step with n_gibbs_steps = 1)
+ *   "x_k" [rows, n_visible], "y_k" [rows, n_classes], "h_k" [rows, n_hidden]   the last sweep's operands
+ *   "aH"  [rows, n_hidden]            w_r h_k (w_r = alpha, or beta on unlabelled rows), the negated dW operand
+ * BM_EINVAL for an unknown name, a size other than rows * width * element size, a chain buffer the step did not write, or
+ * when no step ran since the engine was created or last called predict_proba / transform. */
+int  bm_crbm_debug_last_step(bm_crbm* crbm, const char* name, void* host, size_t bytes);
 int  bm_crbm_predict_proba(bm_crbm* crbm, const void* X, int32_t rows, float* out);    /* p(y|x): out [rows, n_classes] */
 int  bm_crbm_transform(bm_crbm* crbm, const void* X, int32_t rows, float* out);        /* E[h|x]: out [rows, n_hidden]  */
 
