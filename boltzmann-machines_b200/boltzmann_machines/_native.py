@@ -31,7 +31,7 @@ EXPORTS = (
     'bm_dbm_create', 'bm_dbm_destroy', 'bm_dbm_set_param', 'bm_dbm_get_param', 'bm_dbm_init_particles',
     'bm_dbm_train_step', 'bm_dbm_val_metrics', 'bm_dbm_transform', 'bm_dbm_reconstruct', 'bm_dbm_log_proba',
     'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows', 'bm_dbm_pt_counts', 'bm_debug_dbm_multinomial_rows',
-    'bm_dbm_train_step_labeled', 'bm_dbm_predict_proba',
+    'bm_dbm_train_step_labeled', 'bm_dbm_predict_proba', 'bm_dbm_fill', 'bm_dbm_debug_last_fill',
     'bm_crbm_create', 'bm_crbm_destroy', 'bm_crbm_set_param', 'bm_crbm_get_param', 'bm_crbm_init_weights',
     'bm_crbm_train_step', 'bm_crbm_predict_proba', 'bm_crbm_transform', 'bm_crbm_debug_last_step',
     'bm_rbm_group_create', 'bm_rbm_group_destroy', 'bm_rbm_group_train_epoch', 'bm_rbm_group_train_epoch_u8',
@@ -168,6 +168,8 @@ def load_library(path=None):
         'bm_dbm_pt_counts': [vp, vp, vp],
         'bm_dbm_train_step_labeled': [vp, vp, vp, i32, dbl, dbl, i32, u64, u32, i32, C.POINTER(dbl)],
         'bm_dbm_predict_proba': [vp, vp, i32, vp],
+        'bm_dbm_fill': [vp, vp, vp, vp, i32, u32, i32, u64, u32, vp],
+        'bm_dbm_debug_last_fill': [vp, C.c_char_p, vp, sz],
         'bm_debug_dbm_multinomial_rows': [vp, vp, i32, i32, dbl, i32, u64, u32, u32, u32, vp, vp, vp, vp],
         'bm_crbm_create': [vp, C.POINTER(CrbmCfg), C.POINTER(vp)],
         'bm_crbm_set_param': [vp, C.c_char_p, vp, sz], 'bm_crbm_get_param': [vp, C.c_char_p, vp, sz],
@@ -921,6 +923,43 @@ class CudaDBM(object):
         out = np.empty((self.M, self.V), dtype=self.dt)
         check(self._lib.bm_dbm_sample_v(self.handle, int(k), int(seed), int(tick), out.ctypes.data))
         return out
+
+    def fill(self, X, mask, labels=None, row0=0, k=1, seed=0, tick=0):
+        """Clamped Gibbs chains (DESIGN.md §5.9): the visible means of X's rows after ``k`` sweeps with the units where
+        ``mask`` is 1 held at X; these are rows row0.. of the caller's call.  ``labels`` (classification DBMs): [rows] ints
+        in [-1, n_classes), -1 leaving the label free.  Leaves every variable as it was."""
+        X = self._batch(X)
+        m = np.ascontiguousarray(mask, dtype=np.uint8)
+        if m.shape != X.shape:
+            raise ValueError('mask has shape {0}, expected {1}'.format(m.shape, X.shape))
+        y, yp = None, None
+        if labels is not None:
+            y = np.ascontiguousarray(labels, dtype=np.int32).reshape(-1)
+            if y.shape[0] != X.shape[0]:
+                raise ValueError('{0} labels for {1} rows'.format(y.shape[0], X.shape[0]))
+            yp = y.ctypes.data
+        out = np.empty(X.shape, dtype=self.dt)
+        check(self._lib.bm_dbm_fill(self.handle, X.ctypes.data, m.ctypes.data, yp, X.shape[0], int(row0), int(k), int(seed),
+                                    int(tick), out.ctypes.data))
+        return out
+
+    def debug_last_fill(self, name, rows):
+        """one chain state of the last ``fill`` (include/bm.h bm_dbm_debug_last_fill): float32 values widened from the bf16
+        operands on the tensor-core engine, the model dtype on the CUDA-core engine"""
+        base = name[:-5] if name.endswith('_prev') else name
+        sizes = {'v': self.V, 'mean': self.V, 'y': self.C}
+        sizes.update({'h' + _sfx(i): self.Hs[i] for i in range(self.L)})
+        width = sizes[base]
+        tc = self.compute == 'bf16' and self.dt == np.float32 and self._is_tc()
+        a = np.empty((int(rows), width), dtype=np.uint16 if tc else self.dt)
+        check(self._lib.bm_dbm_debug_last_fill(self.handle, name.encode(), a.ctypes.data, a.nbytes))
+        return (a.astype(np.uint32) << 16).view(np.float32) if tc else a
+
+    def _is_tc(self):
+        """the engine bm_dbm_create picked is the tensor-core one (the rule of DbmTC::supports)"""
+        h_kinds = self.cfg.get('h_kinds', ['bernoulli'] * self.L)
+        return (self.cfg.get('v_kind', 'bernoulli') in ('bernoulli', 'gaussian') and
+                all(k in ('bernoulli', 'multinomial') for k in h_kinds))
 
     def ais(self, n_runs, n_betas, k, seed, first_run=None):
         """log Z estimates of ``n_runs`` AIS runs.  ``first_run=None``: the whole ladder (sharded over the ranks of

@@ -164,6 +164,14 @@ class ClassificationDBM(DBM):
         they were."""
         return self._per_batch(X, self.n_classes_, self._engine.predict_proba, 'predict_proba', np.float32)
 
+    @run_in_tf_session(update_seed=True)
+    def fill_missing(self, X, mask, y=None, n_gibbs_steps=100):
+        """``DBM.fill_missing`` with labels: y [n] in {-1, 0, .., n_classes - 1} (None: all -1).  A row labelled t holds
+        its label at e_t in every sweep, so its chain samples p(v_missing | v_observed, y = t); -1 leaves the label free.
+        Class-conditional generation is ``fill_missing(np.zeros((n, V)), np.zeros((n, V)), y=labels)``."""
+        labels = None if y is None else self._labels(y, len(np.asarray(X)), unlabelled=True)
+        return self._fill(X, mask, labels, n_gibbs_steps)
+
     def predict(self, X):
         """argmax of ``predict_proba``; a tie goes to the lowest class index."""
         return np.argmax(self.predict_proba(X), axis=1)

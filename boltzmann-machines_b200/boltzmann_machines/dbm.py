@@ -379,6 +379,44 @@ class DBM(EnergyBasedModel):
         return v
 
     @run_in_tf_session(update_seed=True)
+    def fill_missing(self, X, mask, n_gibbs_steps=100):
+        """Conditional sampling (DESIGN.md §5.9): fill in the units of X where ``mask`` is 0 with a Gibbs chain that holds
+        the units where it is 1 at X.
+
+        Every row runs its own chain: v starts at X where observed and at the visible mean act(vb) elsewhere, the hidden
+        layers at the mean-field E-step's first pass on it; then ``n_gibbs_steps`` sweeps of the model's sampler (as the
+        persistent chains sweep, with ``sample_v_states`` / ``sample_h_states``), the observed units reset to X after every
+        visible update.  Returns the visible means p(v | h_1) of the last sweep [n, n_visible] in the model's dtype, with the
+        observed units equal to X.  For binary and sigma = 1 Gaussian visibles the chain samples p(v_missing | v_observed);
+        with another sigma the DBM's Gaussian conditionals belong to no joint distribution and it is the engine's Gibbs
+        sampler only.  A row's result depends on its own X, mask and index in X and on the call's seed, not on
+        ``batch_size``.  The model's variables, accumulators and particles stay as they were.
+        """
+        return self._fill(X, mask, None, n_gibbs_steps)
+
+    def _fill(self, X, mask, labels, n_gibbs_steps):
+        X = np.ascontiguousarray(X, dtype=self._np_dtype)
+        if X.ndim != 2 or X.shape[1] != self.n_visible_:
+            raise ValueError('X has shape {0}, expected (n, {1})'.format(X.shape, self.n_visible_))
+        mask = np.asarray(mask)
+        if mask.shape != X.shape:
+            raise ValueError('mask has shape {0}, expected {1}'.format(mask.shape, X.shape))
+        if not np.all((mask == 0) | (mask == 1)):
+            raise ValueError('mask must hold 0 (missing) or 1 (observed) only')
+        if not np.all(np.isfinite(X)):
+            raise ValueError('X must be finite')
+        k = int(n_gibbs_steps)
+        if k < 1:
+            raise ValueError('n_gibbs_steps must be >= 1')
+        mask = np.ascontiguousarray(mask, dtype=np.uint8)
+        out = np.empty_like(X)
+        tick = self._next_tick()
+        for lo, hi in _maybe_bar(batch_bounds(len(X), self.batch_size), self.verbose, leave=False, ncols=64, desc='fill_missing'):
+            out[lo:hi] = self._engine.fill(X[lo:hi], mask[lo:hi], labels=None if labels is None else labels[lo:hi],
+                                           row0=lo, k=k, seed=self._call_seed, tick=tick)
+        return out
+
+    @run_in_tf_session(update_seed=True)
     def log_Z(self, n_betas=100, n_runs=100, n_gibbs_steps=5):
         """Annealed-importance-sampling estimate of the log partition function (2 binary hidden
         layers; state space h_1 with v and h_2 summed out analytically).

@@ -182,6 +182,62 @@ __global__ void scale_all_kernel(T* p, size_t n, const double* total) {
         p[i] = (T)((double)p[i] / *total);
 }
 
+// ---- clamped Gibbs chains (bm_dbm_fill, DESIGN.md §5.9) ---------------------------------------------------------------
+// The visible clamp: v[r, c] <- X[r, c] wherever mask[r, c] (dense [rows, cols] bytes, 0 / 1) is set.  S is the chain's element
+// type: the storage dtype on the CUDA-core engine, bf16 operands on the tensor-core one.
+template <typename S>
+__global__ void dbm_fill_clamp_kernel(const uint8_t* __restrict__ mask, const S* __restrict__ X, int ldx, S* __restrict__ v, int ldv,
+                                      int rows, int cols) {
+    const size_t n = (size_t)rows * cols;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t r = i / cols, c = i % cols;
+        if (mask[i]) v[r * ldv + c] = X[r * ldx + c];
+    }
+}
+__device__ __forceinline__ float fill_widen(__nv_bfloat16 x) { return __bfloat162float(x); }
+__device__ __forceinline__ float fill_widen(float x) { return x; }
+__device__ __forceinline__ double fill_widen(double x) { return x; }
+// The result of a fill: out[r, c] = mask ? X[r, c] : mean[r, c] (mean: the chain's element type S, widened to the model's T).
+template <typename S, typename T>
+__global__ void dbm_fill_out_kernel(const uint8_t* __restrict__ mask, const T* __restrict__ X, const S* __restrict__ mean, int ldm,
+                                    T* __restrict__ out, int rows, int cols) {
+    const size_t n = (size_t)rows * cols;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t r = i / cols, c = i % cols;
+        out[i] = mask[i] ? X[i] : (T)fill_widen(mean[r * ldm + c]);
+    }
+}
+static inline unsigned fill_grid(int rows, int cols) {
+    const size_t n = (size_t)rows * cols;
+    return (unsigned)std::min<size_t>((n + 255) / 256, 4096);
+}
+template <typename S>
+void launch_dbm_fill_clamp(Ctx* ctx, const uint8_t* mask, const S* X, int ldx, S* v, int ldv, int rows, int cols) {
+    dbm_fill_clamp_kernel<S><<<fill_grid(rows, cols), 256, 0, ctx->stream>>>(mask, X, ldx, v, ldv, rows, cols);
+    count_launch(ctx);
+}
+template <typename S, typename T>
+void launch_dbm_fill_out(Ctx* ctx, const uint8_t* mask, const T* X, const S* mean, int ldm, T* out, int rows, int cols) {
+    dbm_fill_out_kernel<S, T><<<fill_grid(rows, cols), 256, 0, ctx->stream>>>(mask, X, mean, ldm, out, rows, cols);
+    count_launch(ctx);
+}
+
+// What bm_dbm_fill refuses before anything is launched.  C: classes of the label layer (0: none).
+static void check_fill_args(const uint8_t* mask, const int32_t* labels, int rows, int k, int B, int V, int C) {
+    BM_REQUIRE(rows >= 1 && rows <= B, "fill: rows must lie in 1..batch_size (" + std::to_string(rows) + " given)");
+    BM_REQUIRE(k >= 1, "fill: n_gibbs_steps must be >= 1");
+    const size_t n = (size_t)rows * V;
+    for (size_t i = 0; i < n; ++i)
+        if (mask[i] > 1)
+            throw Error(BM_EINVAL, "fill: mask byte " + std::to_string(i % V) + " of row " + std::to_string(i / V) + " is " +
+                                   std::to_string((int)mask[i]) + ", not 0 or 1");
+    if (!labels) return;
+    if (C == 0) throw Error(BM_EINVAL, "this DBM has no label layer (bm_dbm_cfg.n_classes)");
+    for (int r = 0; r < rows; ++r)
+        if (labels[r] < -1 || labels[r] >= C)
+            throw Error(BM_EINVAL, "label " + std::to_string(labels[r]) + " of row " + std::to_string(r) + " is outside [-1, n_classes)");
+}
+
 // ---------------------------------------------------------------------------------------------
 struct DbmBase {
     Ctx* ctx = nullptr;
@@ -202,6 +258,10 @@ struct DbmBase {
         throw Error(BM_EINVAL, "this DBM has no label layer (bm_dbm_cfg.n_classes)");
     }
     virtual void predict_proba(const void*, int, float*) { throw Error(BM_EINVAL, "this DBM has no label layer (bm_dbm_cfg.n_classes)"); }
+    // clamped Gibbs chains (DESIGN.md §5.9): rows of X [rows, V] with mask [rows, V], labels [rows] or NULL -> out [rows, V]
+    virtual void fill(const void* X, const uint8_t* mask, const int32_t* labels, int rows, uint32_t row0, int k, uint64_t seed,
+                      uint32_t tick, void* out) = 0;
+    virtual void fill_debug(const char* name, void* host, size_t bytes) = 0;
 };
 
 // Parallel tempering (bm_dbm_cfg.n_temps / betas): what the engines refuse before anything is allocated.  0 / NULL is off.
@@ -599,6 +659,68 @@ struct Dbm : DbmBase {
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
     }
 
+    // ---- clamped Gibbs chains (DESIGN.md §5.9) ---------------------------------------------------------------------------
+    // Scratch of its own ([batch_size, n] per layer, allocated on first use): two chain states per layer -- index t % 2 holds
+    // sweep t, 0 the start -- the batch, its mask and the visible means.  Nothing the model or the particles hold is touched.
+    DevBuf<T> fX, fmean, fout, fv[2];
+    std::vector<DevBuf<T>> fh[2];
+    DevBuf<uint8_t> fmask;
+    int f_rows = 0, f_k = 0;                     // the last fill (0: none yet)
+    void fill(const void* Xh, const uint8_t* mask, const int32_t* labels, int rows, uint32_t row0, int k, uint64_t seed,
+              uint32_t tick, void* out) override {
+        check_fill_args(mask, labels, rows, k, B, V, 0);
+        if (fh[0].empty()) {
+            for (DevBuf<T>* b : {&fX, &fmean, &fout, &fv[0], &fv[1]}) b->ensure((size_t)B * V);
+            fmask.ensure((size_t)B * V);
+            for (int s = 0; s < 2; ++s) { fh[s].resize(L); for (int i = 0; i < L; ++i) fh[s][i].ensure((size_t)B * Hs[i]); }
+        }
+        f_rows = 0;
+        BM_CUDA(cudaMemcpyAsync(fX.p, Xh, (size_t)rows * V * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+        BM_CUDA(cudaMemcpyAsync(fmask.p, mask, (size_t)rows * V, cudaMemcpyHostToDevice, ctx->stream));
+        // start: v0 = X where observed, the visible mean with nothing above it (act(0 W_0' + b)) elsewhere
+        BM_CUDA(cudaMemsetAsync(fh[1][0].p, 0, (size_t)rows * Hs[0] * sizeof(T), ctx->stream));
+        visible_op(fh[1][0].p, fv[0].p, nullptr, false, rows, RngKey{});
+        launch_dbm_fill_clamp<T>(ctx, fmask.p, fX.p, V, fv[0].p, V, rows, V);
+        for (int i = 0; i < L; ++i) {                // h0: the E-step's approximate-inference pass on v0 (dbm.py:434-446)
+            const T sc = (i == 0 || i < L - 1) ? T(2) : T(1);
+            hidden_op(i, i == 0 ? fv[0].p : fh[0][i - 1].p, nullptr, fh[0][i].p, nullptr, false, rows, sc, T(1), RngKey{});
+        }
+        for (int t = 1; t <= k; ++t) {               // the particle sweep of gibbs_step, drawing at rows row0 + r
+            const int c = (t - 1) & 1, n = t & 1;
+            for (int i = 0; i < L; ++i) {
+                const T* below = i == 0 ? fv[c].p : fh[n][i - 1].p;
+                const T* above = (i + 1 < L) ? fh[c][i + 1].p : nullptr;
+                hidden_op(i, below, above, fh[n][i].p, fh[n][i].p, sample_h[i] != 0, rows, T(1), T(1), make_rng(seed, SITE_DBM_H + i, t, tick, row0));
+            }
+            visible_op(fh[n][0].p, fv[n].p, fv[n].p, sample_vis != 0, rows, make_rng(seed, SITE_DBM_V, t, tick, row0));
+            launch_dbm_fill_clamp<T>(ctx, fmask.p, fX.p, V, fv[n].p, V, rows, V);
+        }
+        visible_op(fh[k & 1][0].p, fmean.p, nullptr, false, rows, RngKey{});        // p(v | h_1 of the last sweep)
+        launch_dbm_fill_out<T, T>(ctx, fmask.p, fX.p, fmean.p, V, fout.p, rows, V);
+        BM_CUDA(cudaMemcpyAsync(out, fout.p, (size_t)rows * V * sizeof(T), cudaMemcpyDeviceToHost, ctx->stream));
+        BM_CUDA(cudaStreamSynchronize(ctx->stream));
+        f_rows = rows; f_k = k;
+    }
+    // "v", "h", "h_1", ...: the last sweep; the same with "_prev": the sweep before it (the start after one sweep); "mean": the
+    // visible means before the observed units are put back.  [rows, n] in the storage dtype.
+    void fill_debug(const char* name, void* host, size_t bytes) override {
+        BM_REQUIRE(f_rows > 0, "fill_debug: no fill has run on this DBM");
+        std::string n(name);
+        int which = f_k & 1;
+        const std::string suffix = "_prev";
+        if (n.size() > suffix.size() && n.compare(n.size() - suffix.size(), suffix.size(), suffix) == 0) {
+            n = n.substr(0, n.size() - suffix.size()); which = 1 - which;
+        }
+        const T* src = nullptr; int width = 0;
+        if (n == "v") { src = fv[which].p; width = V; }
+        else if (n == "mean" && std::string(name) == "mean") { src = fmean.p; width = V; }
+        else for (int i = 0; i < L; ++i) if (n == "h" + sfx(i)) { src = fh[which][i].p; width = Hs[i]; }
+        BM_REQUIRE(src, std::string("fill_debug: unknown name '") + name + "'");
+        BM_REQUIRE(bytes == (size_t)f_rows * width * sizeof(T), std::string("fill_debug: size mismatch for '") + name + "'");
+        BM_CUDA(cudaMemcpyAsync(host, src, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        BM_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
+
     // ---- AIS (dbm.py:650-736) ---------------------------------------------------------------------------------
     // The runs are independent chains: run r draws from row r of the AIS sites whichever rank or call computes it
     // (row0 = first_run), so a ladder sharded over ranks, or cut into several calls, reproduces the unsharded one.
@@ -802,6 +924,15 @@ int bm_dbm_ais_rows(bm_dbm* h, int32_t n_runs, int32_t n_betas, int32_t k, uint6
 }
 int bm_dbm_pt_counts(bm_dbm* h, int64_t* accepted, int64_t* proposed) {
     BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(accepted && proposed, "null argument"); DBM(h)->pt_counts(accepted, proposed); BM_API_END
+}
+int bm_dbm_fill(bm_dbm* h, const void* X, const uint8_t* mask, const int32_t* labels, int32_t rows, uint32_t row0,
+                int32_t n_gibbs_steps, uint64_t seed, uint32_t tick, void* out) {
+    BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(X && mask && out, "null argument");
+    DBM(h)->fill(X, mask, labels, rows, row0, n_gibbs_steps, seed, tick, out);
+    BM_API_END
+}
+int bm_dbm_debug_last_fill(bm_dbm* h, const char* name, void* host, size_t bytes) {
+    BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(name && host, "null argument"); DBM(h)->fill_debug(name, host, bytes); BM_API_END
 }
 
 int bm_debug_dbm_multinomial_rows(bm_ctx* hctx, const float* pre, int32_t rows, int32_t cols, double n_samples, int32_t n_draws,

@@ -468,8 +468,9 @@ struct DbmTC : Dbm<float> {
     // program, exactly as the ops were listed.
     // cut: the launch ends after this op even without a row kernel (tempered chains longer than one program)
     // clamp: after the row kernel, the rows of `out` labelled >= 0 in this device array are set to their one-hot label
+    // vmask: then the visible clamp of a fill chain (DESIGN.md §5.9): vout <- vx wherever vmask ([rows, V] bytes) is set
     struct RowStep { int layer = -1; bf16_t* out = nullptr; float* out_f32 = nullptr; int rows = 0; bool sample = false; uint32_t site = 0, t = 0; bool cut = false;
-                     const int* clamp = nullptr; };
+                     const int* clamp = nullptr; const uint8_t* vmask = nullptr; const bf16_t* vx = nullptr; bf16_t* vout = nullptr; };
     struct TcChain { std::vector<std::unique_ptr<TcProgram>> progs; std::vector<RowStep> after; };
     // mean-field as persistent dataflow programs of up to MF_CHUNK speculated sweeps per launch: slot history + programs
     static constexpr int MF_CHUNK = 5;
@@ -787,14 +788,16 @@ struct DbmTC : Dbm<float> {
         }
     }
     // the programs get `rng` (seed / tick / row0 shared by their ops); a sampling row kernel draws from (seed, site, t, tick)
+    // at the same first row
     void run_chain(TcChain& chain, RngKey rng, uint64_t seed, uint32_t tick) {
         for (size_t k = 0; k < chain.progs.size(); ++k) {
             launch_tc_program(ctx, *chain.progs[k], rng, 0);
             const RowStep& st = chain.after[k];
             if (st.layer >= 0)
                 multinomial_rows(st.layer, st.rows, st.out, st.out_f32, st.sample,
-                                 st.sample ? make_rng(seed, st.site, st.t, tick, particle_row0()) : RngKey{});
+                                 st.sample ? make_rng(seed, st.site, st.t, tick, rng.row0) : RngKey{});
             if (st.clamp) launch_cdbm_clamp_labels(ctx, st.clamp, st.rows, Hs[st.layer], st.out, ldn[st.layer + 1]);
+            if (st.vmask) launch_dbm_fill_clamp<bf16_t>(ctx, st.vmask, st.vx, ldn[0], st.vout, ldn[0], st.rows, V);
         }
     }
 
@@ -1250,6 +1253,118 @@ struct DbmTC : Dbm<float> {
         particles_f32_stale = true;
         widen_particles();
         BM_CUDA(cudaMemcpyAsync(out, v.p, (size_t)M * V * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+        BM_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
+
+    // ---- clamped Gibbs chains (DESIGN.md §5.9) ---------------------------------------------------------------------------
+    // The chain of particles_program on scratch of its own: index t % 2 of fv_b / fh_b holds sweep t (0: the start).  A sweep is
+    // L hidden ops and the visible op, cut after the visible op for the clamp (dbm_fill_clamp_kernel blends the batch's bf16
+    // operand into v under the mask), so every sweep is one program launch -- plus the row kernels of multinomial layers and,
+    // on a classification DBM with labelled rows, the label clamp after the label's row kernel.  The last sweep also computes
+    // the visible means p(v | h_1) (one more op in its program).  Programs are cached by (rows, sweeps, label clamp).
+    DevBuf<float> fX_f, fout_f;
+    DevBuf<bf16_t> fXb, fmean_b, fv_b[2];
+    std::vector<DevBuf<bf16_t>> fh_b[2];
+    DevBuf<uint8_t> fmask_d;
+    DevBuf<int> flab;
+    std::map<std::tuple<int, int, int>, TcChain> fill_progs;
+    void fill(const void* Xh, const uint8_t* mask, const int32_t* labels, int rows, uint32_t row0, int k, uint64_t seed,
+              uint32_t tick, void* out) override {
+        check_fill_args(mask, labels, rows, k, B, V, top_is_label ? Hs[L - 1] : 0);
+        int labelled = 0;
+        if (labels) for (int r = 0; r < rows; ++r) labelled += labels[r] >= 0;
+        if (fh_b[0].empty()) {
+            fX_f.ensure((size_t)B * V); fout_f.ensure((size_t)B * V); fmask_d.ensure((size_t)B * V);
+            for (DevBuf<bf16_t>* b : {&fXb, &fmean_b, &fv_b[0], &fv_b[1]}) { b->ensure((size_t)B * ldn[0]); b->zero(ctx->stream); }
+            for (int s = 0; s < 2; ++s) {
+                fh_b[s].resize(L);
+                for (int i = 0; i < L; ++i) { fh_b[s][i].ensure((size_t)B * ldn[i + 1]); fh_b[s][i].zero(ctx->stream); }
+            }
+            if (top_is_label) flab.ensure(B);
+        }
+        f_rows = 0;
+        BM_CUDA(cudaMemcpyAsync(fX_f.p, Xh, (size_t)rows * V * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+        BM_CUDA(cudaMemcpyAsync(fmask_d.p, mask, (size_t)rows * V, cudaMemcpyHostToDevice, ctx->stream));
+        if (labelled) BM_CUDA(cudaMemcpyAsync(flab.p, labels, (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+        launch_f32_to_bf16(ctx, fX_f.p, V, fXb.p, ldn[0], rows, V);
+        // start: v0 = X where observed, act(0 W_0' + b) elsewhere; h0 from the E-step's approximate-inference pass (dbm.py:434-446)
+        BM_CUDA(cudaMemsetAsync(fh_b[1][0].p, 0, (size_t)rows * ldn[1] * sizeof(bf16_t), ctx->stream));
+        visible_tc(fh_b[1][0].p, fv_b[0].p, false, rows, RngKey{});
+        launch_dbm_fill_clamp<bf16_t>(ctx, fmask_d.p, fXb.p, ldn[0], fv_b[0].p, ldn[0], rows, V);
+        for (int i = 0; i < L; ++i) {
+            const float sc = (i == 0 || i < L - 1) ? 2.f : 1.f;
+            hidden_tc(i, i == 0 ? fv_b[0].p : fh_b[0][i - 1].p, nullptr, fh_b[0][i].p, false, rows, sc, 1.f, RngKey{});
+            if (labelled && top_is_label && i == L - 1) launch_cdbm_clamp_labels(ctx, flab.p, rows, Hs[i], fh_b[0][i].p, ldn[i + 1]);
+        }
+        TcChain& chain = fill_progs[std::make_tuple(rows, k, labelled ? 1 : 0)];
+        if (chain.progs.empty()) {
+            std::vector<TcGemm> ops;
+            std::vector<RowStep> row;
+            for (int t = 1; t <= k; ++t) {
+                const int c = (t - 1) & 1, n = t & 1;
+                int prev = -1, first = -1;                       // this sweep's op of layer i - 1 / of layer 0
+                for (int i = 0; i < L; ++i) {
+                    const bf16_t* below = i == 0 ? fv_b[c].p : fh_b[n][i - 1].p;
+                    const bf16_t* above = (i + 1 < L) ? fh_b[c][i + 1].p : nullptr;
+                    TcGemm g = hidden_gemm(i, below, above, fh_b[n][i].p, sample_h[i] != 0, rows, 1.f, 1.f,
+                                           make_rng(0, SITE_DBM_H + i, (uint32_t)t, 0, 0));
+                    if (prev >= 0) { g.dep[g.n_deps] = prev; g.dep_all[g.n_deps] = false; ++g.n_deps; }
+                    g.lane = LANE_CHAIN;
+                    prev = (int)ops.size();
+                    if (i == 0) first = prev;
+                    ops.push_back(g);
+                    RowStep st;
+                    if (multinomial(i)) {
+                        st.layer = i; st.out = fh_b[n][i].p; st.rows = rows; st.sample = sample_h[i] != 0;
+                        st.site = SITE_DBM_H + i; st.t = (uint32_t)t;
+                    }
+                    if (labelled && top_is_label && i == L - 1) st.clamp = flab.p;
+                    row.push_back(st);
+                }
+                TcGemm gv = visible_gemm(fh_b[n][0].p, fv_b[n].p, sample_vis != 0, rows, make_rng(0, SITE_DBM_V, (uint32_t)t, 0, 0));
+                gv.dep[0] = first; gv.dep_all[0] = false; gv.n_deps = 1;
+                gv.lane = LANE_CHAIN;
+                ops.push_back(gv);
+                row.push_back(RowStep());
+                if (t == k) {                                    // p(v | h_1) of the last sweep
+                    TcGemm gm = visible_gemm(fh_b[n][0].p, fmean_b.p, false, rows, RngKey{});
+                    gm.dep[0] = first; gm.dep_all[0] = false; gm.n_deps = 1;
+                    gm.lane = LANE_CHAIN;
+                    ops.push_back(gm);
+                    row.push_back(RowStep());
+                }
+                RowStep& end = row.back();                       // the visible clamp ends the sweep's launch
+                end.vmask = fmask_d.p; end.vx = fXb.p; end.vout = fv_b[n].p; end.rows = rows; end.cut = true;
+            }
+            cut_chain(chain, ops, row);
+        }
+        run_chain(chain, make_rng(seed, 0, 0, tick, row0), seed, tick);
+        launch_dbm_fill_out<bf16_t, float>(ctx, fmask_d.p, fX_f.p, fmean_b.p, ldn[0], fout_f.p, rows, V);
+        BM_CUDA(cudaMemcpyAsync(out, fout_f.p, (size_t)rows * V * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+        BM_CUDA(cudaStreamSynchronize(ctx->stream));
+        f_rows = rows; f_k = k;
+    }
+    // as Dbm<T>::fill_debug, as bf16 bit patterns; on a classification DBM the label layer is "y" / "y_prev"
+    void fill_debug(const char* name, void* host, size_t bytes) override {
+        BM_REQUIRE(f_rows > 0, "fill_debug: no fill has run on this DBM");
+        std::string n(name);
+        int which = f_k & 1;
+        const std::string suffix = "_prev";
+        if (n.size() > suffix.size() && n.compare(n.size() - suffix.size(), suffix.size(), suffix) == 0) {
+            n = n.substr(0, n.size() - suffix.size()); which = 1 - which;
+        }
+        const bf16_t* src = nullptr; int width = 0, ld = 0;
+        if (n == "v") { src = fv_b[which].p; width = V; ld = ldn[0]; }
+        else if (n == "mean" && std::string(name) == "mean") { src = fmean_b.p; width = V; ld = ldn[0]; }
+        else
+            for (int i = 0; i < L; ++i) {
+                const bool label = top_is_label && i == L - 1;
+                if (n == (label ? std::string("y") : "h" + sfx(i))) { src = fh_b[which][i].p; width = Hs[i]; ld = ldn[i + 1]; }
+            }
+        BM_REQUIRE(src, std::string("fill_debug: unknown name '") + name + "'");
+        BM_REQUIRE(bytes == (size_t)f_rows * width * sizeof(bf16_t), std::string("fill_debug: size mismatch for '") + name + "'");
+        BM_CUDA(cudaMemcpy2DAsync(host, (size_t)width * sizeof(bf16_t), src, (size_t)ld * sizeof(bf16_t), (size_t)width * sizeof(bf16_t),
+                                  f_rows, cudaMemcpyDeviceToHost, ctx->stream));
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
     }
 

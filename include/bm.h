@@ -277,6 +277,25 @@ int  bm_dbm_ais_rows(bm_dbm* dbm, int32_t n_runs, int32_t n_betas, int32_t n_gib
 /* parallel tempering: swaps accepted / proposed between slots m and m+1 since create, n_temps-1 entries each (BM_EINVAL
  * without tempering) */
 int  bm_dbm_pt_counts(bm_dbm* dbm, int64_t* accepted, int64_t* proposed);
+/* Conditional sampling with clamped Gibbs chains (DESIGN.md §5.9; not in the reference): fill in the missing visible units of
+ * X [rows, n_visible] (model dtype), mask [rows, n_visible] bytes (1: observed, clamped to X; 0: missing, X ignored).  Per row:
+ * v0 = X where observed and act(b) (the visible mean with nothing above) elsewhere; h0 from the mean-field E-step's
+ * approximate-inference pass on v0; then n_gibbs_steps >= 1 particle sweeps (h_1 .. h_L bottom-up, then v), drawing at sites
+ * 16 + i / 11, sweep index t = 1.., the call's seed and tick and row row0 + r, with v reset to X where observed after every
+ * visible update.  out [rows, n_visible] = the visible means p(v | h_1) of the last sweep, X where observed.  A row's result
+ * depends on its X, mask, label and global index row0 + r only, so a caller may cut a call into pieces.  Classification DBM:
+ * labels [rows] in [-1, n_classes) (NULL: all -1); a row labelled t >= 0 holds its label at e_t throughout (the class-
+ * conditional chain), -1 leaves it free.  Reads W and b only: no variable, accumulator, particle, offset or counter changes.
+ * BM_EINVAL before any launch: a null pointer, rows outside 1..batch_size, n_gibbs_steps < 1, a mask byte other than 0 / 1,
+ * a label outside [-1, n_classes), labels on a DBM without a label layer. */
+int  bm_dbm_fill(bm_dbm* dbm, const void* X, const uint8_t* mask, const int32_t* labels, int32_t rows, uint32_t row0,
+                 int32_t n_gibbs_steps, uint64_t seed, uint32_t tick, void* out);
+/* test hook: one chain state of the last bm_dbm_fill, [rows, n] row-major without padding (rows: that call's).  "v", "h",
+ * "h_1", ... (a classification DBM's label layer: "y"): the last sweep; the same names + "_prev": the sweep before it (the start
+ * after one sweep); "mean": the visible means before the observed units are put back.  Elements: bf16 bit patterns (uint16) on
+ * the tensor-core engine, the model dtype on the CUDA-core engine.  Device-to-host copies only.  BM_EINVAL for an unknown name,
+ * a wrong size, or before the first fill. */
+int  bm_dbm_debug_last_fill(bm_dbm* dbm, const char* name, void* host, size_t bytes);
 
 /* ---- test hook: the raw tensor-core GEMM (no counterpart in the reference) -----------------
  * C[M,N] (fp32) = A * B^T (+/- A2 * B2^T), operands given as host fp32 and rounded to bf16.
