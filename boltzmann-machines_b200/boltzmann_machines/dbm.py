@@ -418,14 +418,20 @@ class DBM(EnergyBasedModel):
 
     @run_in_tf_session(update_seed=True)
     def log_Z(self, n_betas=100, n_runs=100, n_gibbs_steps=5):
-        """Annealed-importance-sampling estimate of the log partition function (2 binary hidden
-        layers; state space h_1 with v and h_2 summed out analytically).
+        """Annealed-importance-sampling estimate of the log partition function of a binary DBM.
+
+        The chains run over the odd hidden layers h_1, h_3, ...; v and the even layers are summed out analytically
+        (DESIGN.md §5.4c).  Two hidden layers run on either engine.  Any other number of layers runs on the tensor-core
+        engine (float32 models, ``compute='bf16'``), with the odd layers sampled (``sample_h_states``); otherwise
+        ``NotImplementedError`` names what is missing.  Tempered and centered models need nothing extra.
 
         Returns ``log_mean, (log_low, log_high), values``: log of the mean estimate, of the mean
         minus / plus one standard deviation, and the ``n_runs`` individual estimates.
         """
-        assert self.n_layers_ == 2
-        assert self.layers_['v']['kind'] == 'bernoulli' and all(h['kind'] == 'bernoulli' for h in self.layers_['h'])
+        if self.n_layers_ == 2:
+            assert self.layers_['v']['kind'] == 'bernoulli' and all(h['kind'] == 'bernoulli' for h in self.layers_['h'])
+        else:
+            self._check_depth('log_Z', ais=True)
         ais_seed = self.make_random_seed()           # dbm.py:701
         values = self._engine.ais(int(n_runs), int(n_betas), int(n_gibbs_steps), ais_seed)
         log_mean = log_mean_exp(values)
@@ -436,8 +442,25 @@ class DBM(EnergyBasedModel):
 
     @run_in_tf_session()
     def log_proba(self, X_test, log_Z):
-        """Variational lower bound on log p(v) for the rows of ``X_test`` given an estimate of log Z."""
-        assert self.n_layers_ == 2
-        assert self.layers_['v']['kind'] == 'bernoulli' and all(h['kind'] == 'bernoulli' for h in self.layers_['h'])
+        """Variational lower bound on log p(v) for the rows of ``X_test`` given an estimate of log Z.
+
+        Two hidden layers run on either engine; any other number of binary layers on the tensor-core engine (float32
+        models, ``compute='bf16'``), as for `log_Z`."""
+        if self.n_layers_ == 2:
+            assert self.layers_['v']['kind'] == 'bernoulli' and all(h['kind'] == 'bernoulli' for h in self.layers_['h'])
+        else:
+            self._check_depth('log_proba', ais=False)
         P = self._per_batch(X_test, 0, self._engine.log_proba, 'log_proba', np.float64)
         return P - log_Z
+
+    def _check_depth(self, what, ais):
+        """The refusals of the engine (include/bm.h, bm_dbm_ais / bm_dbm_log_proba) at a depth other than 2."""
+        where = '{0} at {1} hidden layers'.format(what, self.n_layers_)
+        if self.layers_['v']['kind'] != 'bernoulli' or any(h['kind'] != 'bernoulli' for h in self.layers_['h']):
+            raise NotImplementedError(where + ' is defined for binary layers (Bernoulli visible and hidden units)')
+        if np.dtype(self.dtype) != np.float32:
+            raise NotImplementedError(where + ' runs on the tensor-core engine: float32 models only')
+        if getattr(self._engine, 'compute', 'bf16') != 'bf16':
+            raise NotImplementedError(where + " runs on the tensor-core engine, not on the fp32 CUDA-core engine (compute='fp32')")
+        if ais and not all(self.sample_h_states[0::2]):
+            raise NotImplementedError(where + ' needs sampled states in the odd layers h_1, h_3, ... (sample_h_states)')

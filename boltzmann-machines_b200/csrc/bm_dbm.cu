@@ -724,7 +724,7 @@ struct Dbm : DbmBase {
     // ---- AIS (dbm.py:650-736) ---------------------------------------------------------------------------------
     // The runs are independent chains: run r draws from row r of the AIS sites whichever rank or call computes it
     // (row0 = first_run), so a ladder sharded over ranks, or cut into several calls, reproduces the unsharded one.
-    void ais_check(int R, int n_betas, int k) const {
+    virtual void ais_check(int R, int n_betas, int k) const {
         BM_REQUIRE(L == 2 && v_kind == BM_UNIT_BERNOULLI && h_kinds[0] == BM_UNIT_BERNOULLI && h_kinds[1] == BM_UNIT_BERNOULLI,
                    "AIS is defined for a 2-layer binary DBM");
         BM_REQUIRE(R >= 1 && n_betas >= 2 && k >= 1, "bad AIS arguments");
@@ -744,7 +744,9 @@ struct Dbm : DbmBase {
         BM_CUDA(cudaMemcpyAsync(hw.data(), all.p, (size_t)total * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
         // :731-734 -- the reference multiplies by `tf.cast(tf.log(2.), dtype)`: the FLOAT32 value of log 2 in every dtype
-        const double logZ0 = (double)(V + Hs[0] + Hs[1]) * 0.693147182464599609375;
+        int units = V;
+        for (int i = 0; i < L; ++i) units += Hs[i];
+        const double logZ0 = (double)units * 0.693147182464599609375;
         for (int r = 0; r < total; ++r) out[r] = hw[r] + logZ0;
     }
     void ais(int R, int n_betas, int k, uint64_t seed, double* out) override {

@@ -385,6 +385,28 @@ __global__ void ais_fused_step_kernel(double* __restrict__ logw, float a, float 
     if (lane == 0) logw[r] += acc;
 }
 
+// The terms of hidden layer i in the variational bound of a DBM of any depth (dbm.py:743-757 for L layers), in float64 per
+// row: out[r] (+)= t.mu + mu.c + H(clip(mu, 1e-7, 1 - 1e-7)) with t = mu_{i-1} W_i (X W_0 for i = 0); the launch of layer 0
+// also sets out[r] = X.b_v first.  One warp per row, one launch per layer.
+__global__ void dbm_bound_layer_rows_kernel(const float* __restrict__ X, int V, const float* __restrict__ vb,
+                                            const float* __restrict__ mu, const float* __restrict__ t, const float* __restrict__ hb,
+                                            int H, int first, int rows, double* __restrict__ out) {
+    const int r = blockIdx.x * blockDim.y + threadIdx.y;
+    if (r >= rows) return;
+    double a = 0.0;
+    for (int j = threadIdx.x; j < H; j += 32) {
+        const double m = (double)mu[(size_t)r * H + j];
+        a += (double)t[(size_t)r * H + j] * m + m * (double)hb[j];
+        const double s = (double)fminf(fmaxf((float)m, 1e-7f), 1.0f - 1e-7f);
+        a += -s * log(s) - (1.0 - s) * log(1.0 - s);
+    }
+    if (first)
+        for (int j = threadIdx.x; j < V; j += 32) a += (double)X[(size_t)r * V + j] * (double)vb[j];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+    if (threadIdx.x == 0) out[r] = first ? a : out[r] + a;
+}
+
 // ---- parallel tempering: the swap round ------------------------------------------------------------
 // Slot m of the ladder holds rows [m M, (m+1) M) of every bf16 particle buffer x[0] = v, x[1 + i] = h_i.  P[i] [T M, H_i] holds
 // the raw products h_{i-1} W_i + c_i of the same states (one fp32 tensor-core op per layer), so that
@@ -1232,7 +1254,7 @@ struct DbmTC : Dbm<float> {
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
     }
     void log_proba(const void* Xh, int rows, double* out) override {
-        BM_REQUIRE(L == 2, "log_proba is defined for 2 hidden layers");
+        if (L != 2) { log_proba_layers(Xh, rows, out); return; }
         BM_REQUIRE(!multinomial(0) && !multinomial(1), "log_proba is defined for binary hidden layers (dbm.py:946-948)");
         const float* X = upload_tc(Xh, rows);
         mean_field_tc(rows);
@@ -1241,6 +1263,33 @@ struct DbmTC : Dbm<float> {
         dbm_bound_rows_kernel<float><<<(rows + 7) / 8, dim3(32, 8), 0, ctx->stream>>>(X, V, mu[0].p, Hs[0], mu[1].p, Hs[1], t[0].p, t[1].p,
                                                                                      vb.p, hb[0].p, hb[1].p, rows, rowd.p);
         count_launch(ctx);
+        BM_CUDA(cudaMemcpyAsync(out, rowd.p, (size_t)rows * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+        BM_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
+    // AIS and the bound at a depth other than 2 (DESIGN.md §5.4c) are defined for binary layers; the AIS ladder's state ops
+    // also take their linear term from sampled states, so the odd layers h_1, h_3, ... must be sampled
+    void depth_check(bool ais) const {
+        const std::string what = std::string(ais ? "AIS" : "log_proba") + " at " + std::to_string(L) + " hidden layers";
+        bool binary = v_kind == BM_UNIT_BERNOULLI;
+        for (int i = 0; i < L; ++i) binary = binary && h_kinds[i] == BM_UNIT_BERNOULLI;
+        if (!binary) throw Error(BM_EUNSUPPORTED, what + " is defined for binary layers (Bernoulli visible and hidden units)");
+        for (int i = 0; ais && i < L; i += 2)
+            if (!sample_h[i]) throw Error(BM_EUNSUPPORTED, what + " needs sampled states in the odd layers h_1, h_3, ... (sample_h)");
+    }
+    // dbm.py:743-757 for L hidden layers: t_i = mu_{i-1} W_i (X W_0 for i = 0) on the tensor cores, then the row kernel
+    void log_proba_layers(const void* Xh, int rows, double* out) {
+        depth_check(false);
+        const float* X = upload_tc(Xh, rows);
+        mean_field_tc(rows);
+        for (int i = 0; i < L; ++i) {
+            const int in = size_of(i, V, Hs);
+            linear_tc(i == 0 ? Xb.p : mu_b[i - 1].p, ldn[i], rows, in, Wb[i].p, in, Hs[i], ldn[i + 1], true, Hs[i], nullptr, t[i].p);
+        }
+        for (int i = 0; i < L; ++i) {
+            dbm_bound_layer_rows_kernel<<<(rows + 7) / 8, dim3(32, 8), 0, ctx->stream>>>(X, V, vb.p, mu[i].p, t[i].p, hb[i].p, Hs[i],
+                                                                                       i == 0 ? 1 : 0, rows, rowd.p);
+            count_launch(ctx);
+        }
         BM_CUDA(cudaMemcpyAsync(out, rowd.p, (size_t)rows * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
     }
@@ -1383,6 +1432,7 @@ struct DbmTC : Dbm<float> {
     // (145 MB per step at 20 000 runs) never exist; up to 30 steps run as one persistent dataflow launch, every op waiting
     // per 256-run block on the op(s) it reads.  dbm.py:650-736; same draws (sites, ticks, rows) as the kernel-per-pass variant.
     void ais_local(int R, uint32_t row0, int n_betas, int k, uint64_t seed, double* logw_out) override {
+        if (L != 2) { ais_local_layers(R, row0, n_betas, k, seed, logw_out); return; }
         // the transition's epilogue takes the linear term from sampled states
         if (!sample_h[0]) { ais_local_passes(R, row0, n_betas, k, seed, logw_out); return; }
         const int H0 = Hs[0], H1 = Hs[1];
@@ -1452,6 +1502,120 @@ struct DbmTC : Dbm<float> {
         }
         unit_op(true, xc, inc_a(nT - 1), inc_b(nT - 1), true, 0.f, false, 0);      // + log p_M(x_M) - log p_{M-1}(x_M)   :728
         unit_op(false, xc, inc_a(nT - 1), inc_b(nT - 1), true, 0.f, false, 0);
+        // launches of up to TC_PROGRAM_OPS ops; a dependency on an op of an earlier launch is the kernel boundary
+        TcProgram prog;
+        for (size_t lo = 0; lo < all.size(); lo += (size_t)TC_PROGRAM_OPS) {
+            const size_t hi = std::min(all.size(), lo + (size_t)TC_PROGRAM_OPS);
+            prog.ops.assign(all.begin() + lo, all.begin() + hi);
+            for (size_t i = lo; i < hi; ++i) {
+                TcGemm& g = prog.ops[i - lo];
+                g.n_deps = 0;
+                for (int d : {dep0[i], dep1[i]})
+                    if (d >= (int)lo) { g.dep[g.n_deps] = d - (int)lo; g.dep_all[g.n_deps] = false; ++g.n_deps; }
+                g.lane = LANE_ALL;
+            }
+            launch_tc_program(ctx, prog, make_rng(seed, 0, 0, 0, row0), 0);
+        }
+        BM_CUDA(cudaStreamSynchronize(ctx->stream));            // the workspaces above are released on return
+    }
+
+    void ais_check(int R, int n_betas, int k) const override {
+        if (L == 2) { Dbm<float>::ais_check(R, n_betas, k); return; }
+        depth_check(true);
+        BM_REQUIRE(R >= 1 && n_betas >= 2 && k >= 1, "bad AIS arguments");
+    }
+    // The ladder at any other depth (DESIGN.md §5.4c).  Unit layer j = 0..L is v (j = 0) or h_j; the odd layers are the state
+    // x, v and the even layers are summed out: log p*_beta(x) = beta sum_{odd j} c_j.x_j + sum_{even j} sum softplus(beta z_j),
+    // z_j = c_j + x_{j-1} W_{j-1} + x_{j+1} W_j^T.  Per sweep, one ais_kind 1 op per summed-out layer (z_j from its one or two
+    // state neighbours: the weight increment, then the layer's draw at the transition's beta) and one ais_kind 2 op per state
+    // layer (the draw from its one or two summed-out neighbours, plus the linear term): L + 1 ops.  The state layers ping-pong;
+    // every op waits per 256-run block on the last writers of its neighbours, which orders every read of a buffer before the
+    // next write to it.  Draws: v at SITE_AIS_V; hidden layer i = j - 1 at SITE_AIS_H1 (i even) or SITE_AIS_H2 (i odd) with
+    // t = i / 2, its initial state at SITE_AIS_INIT with the same t -- at L = 2 the ladder and the sites of ais_local.
+    void ais_local_layers(int R, uint32_t row0, int n_betas, int k, uint64_t seed, double* logw_out) {
+        const int NL = L + 1;
+        auto width = [&](int j) { return j == 0 ? V : Hs[j - 1]; };
+        auto slot = [&](int j) { return (uint32_t)((j - 1) / 2); };
+        std::vector<DevBuf<bf16_t>> buf(NL), buf2(NL);
+        std::vector<bf16_t*> cur(NL), nxt(NL);
+        for (int j = 0; j < NL; ++j) {
+            buf[j].ensure((size_t)R * ldn[j]); buf[j].zero(ctx->stream);
+            cur[j] = nxt[j] = buf[j].p;
+            if (j % 2) { buf2[j].ensure((size_t)R * ldn[j]); buf2[j].zero(ctx->stream); nxt[j] = buf2[j].p; }
+        }
+        for (int j = 1; j < NL; j += 2) {       // x_0 ~ Ber(1/2)   (:700-702)
+            dim3 g(((width(j) + 3) / 4 + 127) / 128, R);
+            ais_unit_bf16_kernel<<<g, 128, 0, ctx->stream>>>(nullptr, 0, 0.f, cur[j], ldn[j], R, width(j), 1,
+                                                             make_rng(seed, SITE_AIS_INIT, slot(j), 0, row0));
+            count_launch(ctx);
+        }
+        // the temperatures, as ais_local accumulates them
+        const float delta = (float)(1.0 / n_betas);
+        std::vector<float> t;
+        t.push_back(delta);
+        while (t.back() < 1.f - delta + 1e-5f) t.push_back(t.back() + delta);
+        const int nT = (int)t.size();
+        auto inc_a = [&](int j) { return j == 0 ? 0.f : t[j - 1]; };
+        auto inc_b = [&](int j) { return j == nT - 1 ? 1.0f : t[j]; };
+        std::vector<TcGemm> all;
+        std::vector<int> dep0, dep1;                                      // global producer indices (-1: none)
+        std::vector<int> last(NL, -1);                                    // the op that last wrote layer j
+        // z_j from the neighbours of layer j in `x`
+        auto layer_op = [&](int j, const std::vector<bf16_t*>& x) {
+            TcGemm g;
+            g.M = R; g.N = width(j);
+            if (j == 0) {                                                 // x_1 W_0^T: W_0 stored [N, K]
+                g.A[0] = mat(x[1], R, Hs[0], ldn[1]); g.K[0] = Hs[0];
+                g.B[0] = mat(Wb[0].p, V, Hs[0], ldn[1]); g.b_t[0] = false;
+                g.bias = vb.p;
+            } else {                                                      // x_{j-1} W_{j-1} (+ x_{j+1} W_j^T)
+                const int i = j - 1, in = width(j - 1);
+                g.A[0] = mat(x[j - 1], R, in, ldn[j - 1]); g.K[0] = in;
+                g.B[0] = mat(Wb[i].p, in, Hs[i], ldn[j]); g.b_t[0] = true;
+                if (j < L) above_pair(g, i, x[j + 1], R);
+                g.bias = hb[i].p;
+            }
+            dep0.push_back(j >= 1 ? last[j - 1] : -1); dep1.push_back(j + 1 < NL ? last[j + 1] : -1);
+            return g;
+        };
+        auto unit_op = [&](int j, float a, float b, bool weigh, float next, bool emit, uint32_t tick) {
+            TcGemm g = layer_op(j, cur);
+            g.act = ACT_LINEAR;
+            g.ais_kind = 1; g.ais_a = a; g.ais_b = b; g.ais_next = next; g.ais_logw = weigh ? logw_out : nullptr;
+            g.tick_off = tick;
+            if (emit) {
+                const bool smp = j == 0 ? sample_vis != 0 : sample_h[j - 1] != 0;
+                g.sample = smp ? SMP_BERNOULLI : SMP_NONE;
+                g.out_state_bf = cur[j]; g.ld_state_bf = ldn[j];
+                g.rng = j == 0 ? make_rng(0, SITE_AIS_V, 0, 0, 0) : make_rng(0, SITE_AIS_H2, slot(j), 0, 0);
+                last[j] = (int)all.size();
+            }
+            all.push_back(g);
+        };
+        for (int s = 0; s < nT; ++s) {
+            for (int sw = 0; sw < k; ++sw) {
+                const uint32_t tick = (uint32_t)(s * k + sw);
+                const bool weigh = sw == 0 && s >= 1;                    // the increment of x_s (produced by transition s-1)
+                const float a = weigh ? inc_a(s - 1) : 0.f, b = weigh ? inc_b(s - 1) : 0.f;
+                for (int j = 0; j < NL; j += 2) unit_op(j, a, b, weigh, t[s], true, tick);
+                for (int j = 1; j < NL; j += 2) {                         // x'_j ~ sigmoid(beta (z_j - c_j) + beta c_j)
+                    TcGemm o = layer_op(j, cur);
+                    o.acc_scale = t[s]; o.bias_scale = t[s]; o.act = ACT_SIGMOID;
+                    o.sample = SMP_BERNOULLI; o.out_state_bf = nxt[j]; o.ld_state_bf = ldn[j];
+                    o.rng = make_rng(0, SITE_AIS_H1, slot(j), 0, 0);
+                    o.tick_off = tick;
+                    o.ais_kind = 2;
+                    if (sw == k - 1) {
+                        o.ais_logw = logw_out;
+                        o.ais_lin = (float)(((double)inc_b(s) - (double)inc_a(s)) / ((double)t[s] * -1.4426950408889634));
+                    }
+                    last[j] = (int)all.size();
+                    all.push_back(o);
+                    std::swap(cur[j], nxt[j]);                            // the other state ops read summed-out layers only
+                }
+            }
+        }
+        for (int j = 0; j < NL; j += 2) unit_op(j, inc_a(nT - 1), inc_b(nT - 1), true, 0.f, false, 0);    // :728
         // launches of up to TC_PROGRAM_OPS ops; a dependency on an op of an earlier launch is the kernel boundary
         TcProgram prog;
         for (size_t lo = 0; lo < all.size(); lo += (size_t)TC_PROGRAM_OPS) {

@@ -263,12 +263,19 @@ int  bm_dbm_predict_proba(bm_dbm* dbm, const void* X, int32_t rows, float* out);
 int  bm_dbm_val_metrics(bm_dbm* dbm, const void* X, int32_t rows, int32_t n_gibbs_steps, uint64_t seed, uint32_t tick, double* out2);
 int  bm_dbm_transform(bm_dbm* dbm, const void* X, int32_t rows, void* out);       /* mu of the last layer, dbm.py:526-528,859-872 */
 int  bm_dbm_reconstruct(bm_dbm* dbm, const void* X, int32_t rows, void* out);     /* dbm.py:626-632, 874-885 */
-int  bm_dbm_log_proba(bm_dbm* dbm, const void* X, int32_t rows, double* out);     /* variational bound + log Z, dbm.py:738-759 */
+/* The variational bound without -log Z, per row (dbm.py:738-759).  Two hidden layers: either engine.  Any other number of layers:
+ * the tensor-core engine with binary layers only (DESIGN.md §5.4c) -- BM_EUNSUPPORTED for Gaussian visibles or a multinomial
+ * layer; the CUDA-core engine (float64 models, BM_COMPUTE_FP32) keeps its BM_EINVAL refusal. */
+int  bm_dbm_log_proba(bm_dbm* dbm, const void* X, int32_t rows, double* out);
 int  bm_dbm_sample_v(bm_dbm* dbm, int32_t n_gibbs_steps, uint64_t seed, uint32_t tick, void* out);  /* dbm.py:641-648 */
 /* AIS estimates of log Z, one per run (dbm.py:650-736, 899-939).  The runs are independent chains and run r always draws
  * from row r of the AIS sites: on a context with a communicator (bm_ctx_comm_init) the n_runs runs are sharded over the
  * ranks and gathered with one sum-allreduce of n_runs doubles -- every rank calls with the same arguments and receives all
- * n_runs values, identical to a single-GPU call (SURVEY 8e). */
+ * n_runs values, identical to a single-GPU call (SURVEY 8e).  Binary DBMs with two hidden layers run on either engine.  Any
+ * other number of layers runs on the tensor-core engine (DESIGN.md §5.4c: chains over h_1, h_3, ..., with v and the even layers
+ * summed out); there BM_EUNSUPPORTED refuses Gaussian visibles, multinomial layers and an odd layer h_1, h_3, ... that is not
+ * sampled, before any launch.  The CUDA-core engine (float64 models, BM_COMPUTE_FP32) refuses any depth but 2 (BM_EINVAL),
+ * and a classification DBM refuses AIS at every depth (BM_EUNSUPPORTED). */
 int  bm_dbm_ais(bm_dbm* dbm, int32_t n_runs, int32_t n_betas, int32_t n_gibbs_steps, uint64_t seed, double* logZ);
 /* runs [first_run, first_run + n_runs) of the same ladder, no communication: for callers that shard or chunk the runs
  * themselves (one process driving several GPUs; more runs than fit in memory at once) */

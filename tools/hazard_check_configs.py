@@ -1,12 +1,14 @@
 """Dataflow-hazard check of the step programs at BASELINE.json's full sizes, on the host simulation (no GPU):
 
-    python tools/hazard_check_configs.py [cfg2] [cfg3] [cfg4]
+    python tools/hazard_check_configs.py [cfg2] [cfg3] [cfg4] [ais-depth]
 
 Every element a program launch reads or writes is shadowed while the launch is interpreted (tests/hostsim/kernels_cpu.cpp,
 `Hazards`); a read of / write over something another op of the launch touched must be covered by a declared dependency path,
 256-row block by 256-row block.  cfg2: Bernoulli RBM 784-1024, batch 4096, CD-5 (the benchmark's program, 16 row blocks).
 cfg3: Gaussian RBM 3072-5000, batch 512 (host batch and resident-dataset step).  cfg4: the tensor-core DBM engine's mean-field
-and particle programs, 784-512-1024, batch = particles = 1024.  About 3 minutes, 2 GB."""
+and particle programs, 784-512-1024, batch = particles = 1024.  ais-depth (not run by default): the AIS ladders of
+DbmTC::ais_local_layers at one, three and four hidden layers (100-64, 100-64-48-32, 100-64-48-32-16; 600 runs = three 256-run
+blocks, 40 temperatures, k = 2, several launches per ladder).  About 3 minutes, 2 GB."""
 import ctypes as C
 import os
 import subprocess
@@ -75,6 +77,22 @@ def main():
         eng.train_step((rng.rand(B, V) < 0.2).astype(np.float32), 0.01, 0.5, 5, 7, 0)
         ok = report('cfg4 DBM programs') and ok
         eng.close()
+    if 'ais-depth' in which:
+        for Hs in ((64,), (64, 48, 32), (64, 48, 32, 16)):
+            V, L = 100, len(Hs)
+            cfg = dict(n_visible=V, n_hiddens=list(Hs), v_kind='bernoulli', h_kinds=['bernoulli'] * L, dtype='float32',
+                       compute='bf16', n_particles=16, batch_size=16, sample_v=True, sample_h=[True] * L)
+            eng = _native.CudaDBM(cfg)
+            sizes = [V] + list(Hs)
+            d = {'vb': np.zeros(V, np.float32)}
+            for i in range(L):
+                s = '' if i == 0 else '_%d' % i
+                d['W' + s] = (0.1 * rng.randn(sizes[i], sizes[i + 1])).astype(np.float32)
+                d['hb' + s] = np.zeros(sizes[i + 1], np.float32)
+            eng.set_params(d)
+            eng.ais(600, 40, 2, 3)
+            ok = report('AIS ladder at {0} hidden layers'.format(L)) and ok
+            eng.close()
     sys.exit(0 if ok else 1)
 
 
