@@ -30,7 +30,7 @@ EXPORTS = (
     'bm_rbm_get_activation', 'bm_debug_tc_gemm', 'bm_debug_tc_op', 'bm_rbm_debug_tc_plan',
     'bm_dbm_create', 'bm_dbm_destroy', 'bm_dbm_set_param', 'bm_dbm_get_param', 'bm_dbm_init_particles',
     'bm_dbm_train_step', 'bm_dbm_val_metrics', 'bm_dbm_transform', 'bm_dbm_reconstruct', 'bm_dbm_log_proba',
-    'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows', 'bm_dbm_pt_counts', 'bm_debug_dbm_multinomial_rows',
+    'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows', 'bm_dbm_ais_base', 'bm_dbm_ais_base_rows', 'bm_dbm_pt_counts', 'bm_debug_dbm_multinomial_rows',
     'bm_dbm_train_step_labeled', 'bm_dbm_predict_proba', 'bm_dbm_fill', 'bm_dbm_debug_last_fill',
     'bm_crbm_create', 'bm_crbm_destroy', 'bm_crbm_set_param', 'bm_crbm_get_param', 'bm_crbm_init_weights',
     'bm_crbm_train_step', 'bm_crbm_predict_proba', 'bm_crbm_transform', 'bm_crbm_debug_last_step',
@@ -165,6 +165,8 @@ def load_library(path=None):
         'bm_dbm_log_proba': [vp, vp, i32, vp], 'bm_dbm_sample_v': [vp, i32, u64, u32, vp],
         'bm_dbm_ais': [vp, i32, i32, i32, u64, vp],
         'bm_dbm_ais_rows': [vp, i32, i32, i32, u64, u32, vp],
+        'bm_dbm_ais_base': [vp, i32, i32, i32, u64, vp, vp],
+        'bm_dbm_ais_base_rows': [vp, i32, i32, i32, u64, u32, vp, vp],
         'bm_dbm_pt_counts': [vp, vp, vp],
         'bm_dbm_train_step_labeled': [vp, vp, vp, i32, dbl, dbl, i32, u64, u32, i32, C.POINTER(dbl)],
         'bm_dbm_predict_proba': [vp, vp, i32, vp],
@@ -394,15 +396,21 @@ def _round8(n):
 def debug_tc_op(pairs, outputs=('f32',), splits=1, force_bn=0, force_cluster=0, acc_scale=1.0, bias_scale=1.0, bias=None,
                 sigma=None, noise_sigma=None, act='linear', sample=None, seed=0, site=0, t=0, tick=0, row0=0, tick_off=0,
                 ais_kind=0, ais_a=0.0, ais_b=0.0, ais_next=0.0, ais_lin=0.0, logw=None, mean_ld=None, state_ld=None,
-                f32_ld=None, guard_rows=2, ctx=None):
+                f32_ld=None, guard_rows=2, ctx=None, ais_base=None):
     """One fused tensor-core op (test hook, bm_debug_tc_op): C = sum over `pairs` of (+/-) A B^T, then the epilogue.
 
     pairs: 1 or 2 tuples (A, B, a_t, b_t, neg); A is [M,K] (a_t: [K,M]), B is [N,K] (b_t: [K,N]), rounded to bf16 here.
     outputs: any of 'mean', 'state' (bf16) and 'f32'.  Every output buffer has `guard_rows` rows past M and columns past
     round_up(N, 8), is filled with the sentinel bit pattern before the launch and is returned whole: 'mean' / 'state' as
     uint16 bf16 bit patterns [M + guard_rows, ld], 'f32' as float32 [splits, M + guard_rows, ld].  logw (float64 [M]) is
-    added to by the AIS epilogues and returned with one guard entry (LOGW_SENTINEL) past M.  'plan' describes the launch."""
+    added to by the AIS epilogues and returned with one guard entry (LOGW_SENTINEL) past M.  ais_base ([N] or None): the AIS
+    ops' base bias a, added to every sigmoid argument after the beta scaling (it travels in the noise_sigma slot, which AIS ops
+    never use).  'plan' describes the launch."""
     ctx = ctx or Context.default()
+    if ais_base is not None:
+        if not ais_kind or noise_sigma is not None:
+            raise ValueError('ais_base belongs to an AIS op without noise_sigma')
+        noise_sigma = ais_base
     if not 1 <= len(pairs) <= 2:
         raise ValueError('one or two operand pairs')
     a = TcOpArgs()
@@ -961,15 +969,30 @@ class CudaDBM(object):
         return (self.cfg.get('v_kind', 'bernoulli') in ('bernoulli', 'gaussian') and
                 all(k in ('bernoulli', 'multinomial') for k in h_kinds))
 
-    def ais(self, n_runs, n_betas, k, seed, first_run=None):
+    def ais(self, n_runs, n_betas, k, seed, first_run=None, base=None):
         """log Z estimates of ``n_runs`` AIS runs.  ``first_run=None``: the whole ladder (sharded over the ranks of
-        the context's communicator, if any); an integer: runs [first_run, first_run + n_runs) of it, computed here."""
+        the context's communicator, if any); an integer: runs [first_run, first_run + n_runs) of it, computed here.
+        ``base``: None, or one entry per unit layer (v, h_1 .. h_L), each None or the layer's base-rate biases -- the ladder
+        then starts from that factorial model (bm_dbm_ais_base, DESIGN.md §5.4d)."""
         out = np.empty(int(n_runs), dtype=np.float64)
+        bp, keep = None, []
+        if base is not None:
+            if len(base) != self.L + 1:
+                raise ValueError('base needs one entry per unit layer (v, h_1 .. h_L): {0}'.format(self.L + 1))
+            bp = (C.c_void_p * len(base))()
+            for j, a in enumerate(base):
+                if a is None:
+                    continue
+                a = np.ascontiguousarray(a, dtype=np.float32).ravel()
+                if a.size != ([self.V] + self.Hs)[j]:
+                    raise ValueError('base of layer {0} has {1} entries, the layer {2}'.format(j, a.size, ([self.V] + self.Hs)[j]))
+                keep.append(a)
+                bp[j] = a.ctypes.data
         if first_run is None:
-            check(self._lib.bm_dbm_ais(self.handle, int(n_runs), int(n_betas), int(k), int(seed), out.ctypes.data))
+            check(self._lib.bm_dbm_ais_base(self.handle, int(n_runs), int(n_betas), int(k), int(seed), bp, out.ctypes.data))
         else:
-            check(self._lib.bm_dbm_ais_rows(self.handle, int(n_runs), int(n_betas), int(k), int(seed), int(first_run),
-                                            out.ctypes.data))
+            check(self._lib.bm_dbm_ais_base_rows(self.handle, int(n_runs), int(n_betas), int(k), int(seed), int(first_run), bp,
+                                                 out.ctypes.data))
         return out
 
     def close(self):

@@ -417,7 +417,7 @@ class DBM(EnergyBasedModel):
         return out
 
     @run_in_tf_session(update_seed=True)
-    def log_Z(self, n_betas=100, n_runs=100, n_gibbs_steps=5):
+    def log_Z(self, n_betas=100, n_runs=100, n_gibbs_steps=5, base_rate=None):
         """Annealed-importance-sampling estimate of the log partition function of a binary DBM.
 
         The chains run over the odd hidden layers h_1, h_3, ...; v and the even layers are summed out analytically
@@ -425,15 +425,29 @@ class DBM(EnergyBasedModel):
         engine (float32 models, ``compute='bf16'``), with the odd layers sampled (``sample_h_states``); otherwise
         ``NotImplementedError`` names what is missing.  Tempered and centered models need nothing extra.
 
+        ``base_rate`` starts the ladder from a factorial base-rate model instead of the uniform one (DESIGN.md §5.4d;
+        Salakhutdinov & Hinton 2009), which needs far fewer temperatures for a model of data whose units are mostly off:
+          * None: the uniform start;
+          * a training-data array ``X`` [n, n_visible] with values in [0, 1]: visible base biases
+            logit((sum_r X_r + 1) / (n + 2)), hidden layers uniform;
+          * a list or tuple of ``n_layers + 1`` entries (v, h_1 .. h_L), each None (uniform) or the layer's base biases.
+        A base runs on the tensor-core engine at every depth, with the odd layers sampled.
+
         Returns ``log_mean, (log_low, log_high), values``: log of the mean estimate, of the mean
-        minus / plus one standard deviation, and the ``n_runs`` individual estimates.
+        minus / plus one standard deviation, and the ``n_runs`` individual estimates (log Z_A included).
         """
-        if self.n_layers_ == 2:
+        base = self._base_rates(base_rate) if base_rate is not None else None
+        if base is not None:
+            self._check_depth('log_Z from a base-rate model', ais=True)
+        elif self.n_layers_ == 2:
             assert self.layers_['v']['kind'] == 'bernoulli' and all(h['kind'] == 'bernoulli' for h in self.layers_['h'])
         else:
             self._check_depth('log_Z', ais=True)
         ais_seed = self.make_random_seed()           # dbm.py:701
-        values = self._engine.ais(int(n_runs), int(n_betas), int(n_gibbs_steps), ais_seed)
+        if base is None:
+            values = self._engine.ais(int(n_runs), int(n_betas), int(n_gibbs_steps), ais_seed)
+        else:
+            values = self._engine.ais(int(n_runs), int(n_betas), int(n_gibbs_steps), ais_seed, base=base)
         log_mean = log_mean_exp(values)
         log_std = log_std_exp(values, log_mean_exp_x=log_mean)
         log_high = log_sum_exp([log_std, log_mean])
@@ -453,9 +467,36 @@ class DBM(EnergyBasedModel):
         P = self._per_batch(X_test, 0, self._engine.log_proba, 'log_proba', np.float64)
         return P - log_Z
 
+    def _base_rates(self, base_rate):
+        """log_Z's ``base_rate`` as one float32 vector or None per unit layer (v, h_1 .. h_L)"""
+        widths = [self.n_visible_] + [int(n) for n in self.n_hiddens_]
+        if isinstance(base_rate, (list, tuple)):
+            if len(base_rate) != len(widths):
+                raise ValueError('base_rate: {0} per-layer entries (v, h_1 .. h_L), got {1}'.format(len(widths), len(base_rate)))
+            base = []
+            for j, a in enumerate(base_rate):
+                if a is not None:
+                    a = np.asarray(a, dtype=np.float64).ravel()
+                    if a.size != widths[j]:
+                        raise ValueError('base_rate[{0}] has {1} entries, layer {0} has {2} units'.format(j, a.size, widths[j]))
+                    if not np.all(np.isfinite(a)):
+                        raise ValueError('base_rate[{0}] has non-finite entries'.format(j))
+                    a = a.astype(np.float32)
+                base.append(a)
+            return base
+        X = np.asarray(base_rate, dtype=np.float64)
+        if X.ndim != 2 or X.shape[1] != widths[0] or X.shape[0] < 1:
+            raise ValueError('base_rate: data [n, {0}] or {1} per-layer vectors (v, h_1 .. h_L), got shape {2}'.format(
+                widths[0], len(widths), X.shape))
+        if not np.all((X >= 0.) & (X <= 1.)):
+            raise ValueError('base_rate: data values must lie in [0, 1]')
+        p = (X.sum(axis=0) + 1.) / (X.shape[0] + 2.)
+        return [np.log(p / (1. - p)).astype(np.float32)] + [None] * self.n_layers_
+
     def _check_depth(self, what, ais):
-        """The refusals of the engine (include/bm.h, bm_dbm_ais / bm_dbm_log_proba) at a depth other than 2."""
-        where = '{0} at {1} hidden layers'.format(what, self.n_layers_)
+        """The refusals of the engine (include/bm.h, bm_dbm_ais / bm_dbm_ais_base / bm_dbm_log_proba) at a depth other than 2,
+        and of AIS from a base-rate model at any depth."""
+        where = what if 'base-rate' in what else '{0} at {1} hidden layers'.format(what, self.n_layers_)
         if self.layers_['v']['kind'] != 'bernoulli' or any(h['kind'] != 'bernoulli' for h in self.layers_['h']):
             raise NotImplementedError(where + ' is defined for binary layers (Bernoulli visible and hidden units)')
         if np.dtype(self.dtype) != np.float32:

@@ -15,6 +15,8 @@
 // row sums that enter the update (pos^T mu - neg^T h per layer, the column sums of mu, h, X, v) are sum-allreduced
 // in one buffer before every rank applies the identical update.  With one rank nothing below changes.
 #include "bm_rbm.h"
+#include <algorithm>
+#include <cmath>
 #include <vector>
 #include <string>
 
@@ -251,8 +253,9 @@ struct DbmBase {
     virtual void reconstruct(const void* X, int rows, void* out) = 0;
     virtual void log_proba(const void* X, int rows, double* out) = 0;
     virtual void sample_v(int k, uint64_t seed, uint32_t tick, void* out) = 0;
-    virtual void ais(int n_runs, int n_betas, int k, uint64_t seed, double* out) = 0;
-    virtual void ais_rows(int n_runs, int n_betas, int k, uint64_t seed, uint32_t first_run, double* out) = 0;
+    // base: NULL or L + 1 nullable host vectors (v, h_1 .. h_L) of an AIS base-rate model (DESIGN.md §5.4d); all-null is NULL
+    virtual void ais(int n_runs, int n_betas, int k, uint64_t seed, const float* const* base, double* out) = 0;
+    virtual void ais_rows(int n_runs, int n_betas, int k, uint64_t seed, uint32_t first_run, const float* const* base, double* out) = 0;
     virtual void pt_counts(int64_t*, int64_t*) { throw Error(BM_EINVAL, "this DBM has no tempered chains (bm_dbm_cfg.n_temps)"); }
     virtual void train_step_labeled(const void*, const int32_t*, int, double, double, int, uint64_t, uint32_t, int, double*) {
         throw Error(BM_EINVAL, "this DBM has no label layer (bm_dbm_cfg.n_classes)");
@@ -724,13 +727,22 @@ struct Dbm : DbmBase {
     // ---- AIS (dbm.py:650-736) ---------------------------------------------------------------------------------
     // The runs are independent chains: run r draws from row r of the AIS sites whichever rank or call computes it
     // (row0 = first_run), so a ladder sharded over ranks, or cut into several calls, reproduces the unsharded one.
-    virtual void ais_check(int R, int n_betas, int k) const {
+    bool has_base(const float* const* base) const {
+        for (int j = 0; base && j <= L; ++j)
+            if (base[j]) return true;
+        return false;
+    }
+    virtual void ais_check(int R, int n_betas, int k, const float* const* base) const {
+        if (has_base(base))
+            throw Error(BM_EUNSUPPORTED, "AIS from a base-rate model runs on the tensor-core engine (float32 models, BM_COMPUTE_BF16), "
+                                         "not on the CUDA-core engine");
         BM_REQUIRE(L == 2 && v_kind == BM_UNIT_BERNOULLI && h_kinds[0] == BM_UNIT_BERNOULLI && h_kinds[1] == BM_UNIT_BERNOULLI,
                    "AIS is defined for a 2-layer binary DBM");
         BM_REQUIRE(R >= 1 && n_betas >= 2 && k >= 1, "bad AIS arguments");
     }
     // runs [first, first + n) of a ladder of `total` runs -> out[0..n)
-    void ais_slice(int n, uint32_t first, int n_betas, int k, uint64_t seed, double* out, bool reduce, int total, int offset) {
+    void ais_slice(int n, uint32_t first, int n_betas, int k, uint64_t seed, const float* const* base, double* out, bool reduce,
+                   int total, int offset) {
         DevBuf<double> all;
         all.ensure(total);
         all.zero(ctx->stream);
@@ -738,7 +750,7 @@ struct Dbm : DbmBase {
         // chunks -- run r draws from row r whatever the chunking
         const int chunk = 32768;
         for (int done = 0; done < n; done += chunk)
-            ais_local(std::min(chunk, n - done), first + (uint32_t)done, n_betas, k, seed, all.p + offset + done);
+            ais_local(std::min(chunk, n - done), first + (uint32_t)done, n_betas, k, seed, base, all.p + offset + done);
         if (reduce) allreduce_sum(ctx, all.p, (size_t)total, true);        // every rank ends with every run
         std::vector<double> hw(total);
         BM_CUDA(cudaMemcpyAsync(hw.data(), all.p, (size_t)total * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
@@ -746,22 +758,31 @@ struct Dbm : DbmBase {
         // :731-734 -- the reference multiplies by `tf.cast(tf.log(2.), dtype)`: the FLOAT32 value of log 2 in every dtype
         int units = V;
         for (int i = 0; i < L; ++i) units += Hs[i];
-        const double logZ0 = (double)units * 0.693147182464599609375;
+        double logZ0 = (double)units * 0.693147182464599609375;
+        if (has_base(base)) {               // log Z_A = sum_j sum_n softplus(a_{j,n}) in float64 (a layer without a base: a = 0)
+            logZ0 = 0.0;
+            for (int j = 0; j <= L; ++j)
+                for (int c = 0, w = j == 0 ? V : Hs[j - 1]; c < w; ++c) {
+                    const double a = base[j] ? (double)base[j][c] : 0.0;
+                    logZ0 += std::max(a, 0.0) + std::log1p(std::exp(-std::fabs(a)));
+                }
+        }
         for (int r = 0; r < total; ++r) out[r] = hw[r] + logZ0;
     }
-    void ais(int R, int n_betas, int k, uint64_t seed, double* out) override {
-        ais_check(R, n_betas, k);
+    void ais(int R, int n_betas, int k, uint64_t seed, const float* const* base, double* out) override {
+        ais_check(R, n_betas, k, base);
         // with a communicator the runs are sharded over the ranks (SURVEY 8e) and gathered by one sum-allreduce of R doubles
         const int nr = ctx->nranks > 1 ? ctx->nranks : 1, rk = ctx->nranks > 1 ? ctx->rank : 0;
         const int lo = (int)((long long)R * rk / nr), hi = (int)((long long)R * (rk + 1) / nr);
-        ais_slice(hi - lo, (uint32_t)lo, n_betas, k, seed, out, nr > 1, R, lo);
+        ais_slice(hi - lo, (uint32_t)lo, n_betas, k, seed, base, out, nr > 1, R, lo);
     }
-    void ais_rows(int R, int n_betas, int k, uint64_t seed, uint32_t first_run, double* out) override {
-        ais_check(R, n_betas, k);
-        ais_slice(R, first_run, n_betas, k, seed, out, false, R, 0);
+    void ais_rows(int R, int n_betas, int k, uint64_t seed, uint32_t first_run, const float* const* base, double* out) override {
+        ais_check(R, n_betas, k, base);
+        ais_slice(R, first_run, n_betas, k, seed, base, out, false, R, 0);
     }
-    // R chains starting at global run `row0`; their log-weights (without log Z_0) are ADDED to logw_out[0..R) (device, zeroed)
-    virtual void ais_local(int R, uint32_t row0, int n_betas, int k, uint64_t seed, double* logw_out) {
+    // R chains starting at global run `row0`; their log-weights (without log Z_0) are ADDED to logw_out[0..R) (device, zeroed).
+    // This engine has no base (ais_check refuses one).
+    virtual void ais_local(int R, uint32_t row0, int n_betas, int k, uint64_t seed, const float* const*, double* logw_out) {
         const int H0 = Hs[0], H1 = Hs[1];
         DevBuf<T> x, xn, va, hc, pa, pb;
         struct { double* p; } logw{logw_out};
@@ -918,11 +939,18 @@ int bm_dbm_log_proba(bm_dbm* h, const void* X, int32_t rows, double* out) {
 int bm_dbm_sample_v(bm_dbm* h, int32_t k, uint64_t seed, uint32_t tick, void* out) {
     BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(out, "null argument"); DBM(h)->sample_v(k, seed, tick, out); BM_API_END
 }
+int bm_dbm_ais_base(bm_dbm* h, int32_t n_runs, int32_t n_betas, int32_t k, uint64_t seed, const float* const* base, double* logZ) {
+    BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(logZ, "null argument"); DBM(h)->ais(n_runs, n_betas, k, seed, base, logZ); BM_API_END
+}
+int bm_dbm_ais_base_rows(bm_dbm* h, int32_t n_runs, int32_t n_betas, int32_t k, uint64_t seed, uint32_t first_run,
+                         const float* const* base, double* logZ) {
+    BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(logZ, "null argument"); DBM(h)->ais_rows(n_runs, n_betas, k, seed, first_run, base, logZ); BM_API_END
+}
 int bm_dbm_ais(bm_dbm* h, int32_t n_runs, int32_t n_betas, int32_t k, uint64_t seed, double* logZ) {
-    BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(logZ, "null argument"); DBM(h)->ais(n_runs, n_betas, k, seed, logZ); BM_API_END
+    return bm_dbm_ais_base(h, n_runs, n_betas, k, seed, nullptr, logZ);
 }
 int bm_dbm_ais_rows(bm_dbm* h, int32_t n_runs, int32_t n_betas, int32_t k, uint64_t seed, uint32_t first_run, double* logZ) {
-    BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(logZ, "null argument"); DBM(h)->ais_rows(n_runs, n_betas, k, seed, first_run, logZ); BM_API_END
+    return bm_dbm_ais_base_rows(h, n_runs, n_betas, k, seed, first_run, nullptr, logZ);
 }
 int bm_dbm_pt_counts(bm_dbm* h, int64_t* accepted, int64_t* proposed) {
     BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(accepted && proposed, "null argument"); DBM(h)->pt_counts(accepted, proposed); BM_API_END

@@ -1266,10 +1266,12 @@ struct DbmTC : Dbm<float> {
         BM_CUDA(cudaMemcpyAsync(out, rowd.p, (size_t)rows * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
     }
-    // AIS and the bound at a depth other than 2 (DESIGN.md §5.4c) are defined for binary layers; the AIS ladder's state ops
-    // also take their linear term from sampled states, so the odd layers h_1, h_3, ... must be sampled
-    void depth_check(bool ais) const {
-        const std::string what = std::string(ais ? "AIS" : "log_proba") + " at " + std::to_string(L) + " hidden layers";
+    // AIS and the bound at a depth other than 2 (DESIGN.md §5.4c), and AIS from a base-rate model at any depth (§5.4d), are
+    // defined for binary layers; the AIS ladder's state ops also take their linear term from sampled states, so the odd layers
+    // h_1, h_3, ... must be sampled
+    void depth_check(bool ais, bool base = false) const {
+        const std::string what = base ? std::string("AIS from a base-rate model")
+                                      : std::string(ais ? "AIS" : "log_proba") + " at " + std::to_string(L) + " hidden layers";
         bool binary = v_kind == BM_UNIT_BERNOULLI;
         for (int i = 0; i < L; ++i) binary = binary && h_kinds[i] == BM_UNIT_BERNOULLI;
         if (!binary) throw Error(BM_EUNSUPPORTED, what + " is defined for binary layers (Bernoulli visible and hidden units)");
@@ -1431,8 +1433,8 @@ struct DbmTC : Dbm<float> {
     // -- "the same kernel with a scalar beta multiplied into the pre-activation" (north_star).  The fp32 pre-activations
     // (145 MB per step at 20 000 runs) never exist; up to 30 steps run as one persistent dataflow launch, every op waiting
     // per 256-run block on the op(s) it reads.  dbm.py:650-736; same draws (sites, ticks, rows) as the kernel-per-pass variant.
-    void ais_local(int R, uint32_t row0, int n_betas, int k, uint64_t seed, double* logw_out) override {
-        if (L != 2) { ais_local_layers(R, row0, n_betas, k, seed, logw_out); return; }
+    void ais_local(int R, uint32_t row0, int n_betas, int k, uint64_t seed, const float* const* base, double* logw_out) override {
+        if (L != 2 || has_base(base)) { ais_local_layers(R, row0, n_betas, k, seed, base, logw_out); return; }
         // the transition's epilogue takes the linear term from sampled states
         if (!sample_h[0]) { ais_local_passes(R, row0, n_betas, k, seed, logw_out); return; }
         const int H0 = Hs[0], H1 = Hs[1];
@@ -1519,10 +1521,15 @@ struct DbmTC : Dbm<float> {
         BM_CUDA(cudaStreamSynchronize(ctx->stream));            // the workspaces above are released on return
     }
 
-    void ais_check(int R, int n_betas, int k) const override {
-        if (L == 2) { Dbm<float>::ais_check(R, n_betas, k); return; }
-        depth_check(true);
+    void ais_check(int R, int n_betas, int k, const float* const* base) const override {
+        const bool with_base = has_base(base);
+        if (L == 2 && !with_base) { Dbm<float>::ais_check(R, n_betas, k, nullptr); return; }
+        depth_check(true, with_base);
         BM_REQUIRE(R >= 1 && n_betas >= 2 && k >= 1, "bad AIS arguments");
+        for (int j = 0; with_base && j <= L; ++j)
+            for (int c = 0, w = j == 0 ? V : Hs[j - 1]; base[j] && c < w; ++c)
+                if (!std::isfinite(base[j][c]))
+                    throw Error(BM_EINVAL, "AIS base of layer " + std::to_string(j) + " (0: v) has a non-finite entry");
     }
     // The ladder at any other depth (DESIGN.md §5.4c).  Unit layer j = 0..L is v (j = 0) or h_j; the odd layers are the state
     // x, v and the even layers are summed out: log p*_beta(x) = beta sum_{odd j} c_j.x_j + sum_{even j} sum softplus(beta z_j),
@@ -1532,10 +1539,29 @@ struct DbmTC : Dbm<float> {
     // every op waits per 256-run block on the last writers of its neighbours, which orders every read of a buffer before the
     // next write to it.  Draws: v at SITE_AIS_V; hidden layer i = j - 1 at SITE_AIS_H1 (i even) or SITE_AIS_H2 (i odd) with
     // t = i / 2, its initial state at SITE_AIS_INIT with the same t -- at L = 2 the ladder and the sites of ais_local.
-    void ais_local_layers(int R, uint32_t row0, int n_betas, int k, uint64_t seed, double* logw_out) {
+    // With a base-rate model (DESIGN.md §5.4d; base: NULL or L + 1 nullable host vectors a_j) the path runs from
+    // p_A ∝ exp(sum_j a_j.x_j): every op reads u_j = z_j - a_j, i.e. the bias b_j - a_j, and adds a_j after the beta scaling in
+    // its epilogue (TcGemm::ais_base); the initial states are drawn from sigmoid(a_j).
+    void ais_local_layers(int R, uint32_t row0, int n_betas, int k, uint64_t seed, const float* const* base, double* logw_out) {
         const int NL = L + 1;
         auto width = [&](int j) { return j == 0 ? V : Hs[j - 1]; };
         auto slot = [&](int j) { return (uint32_t)((j - 1) / 2); };
+        std::vector<const float*> bias(NL), abase(NL, nullptr);
+        std::vector<DevBuf<float>> a_dev(NL), d_dev(NL);
+        std::vector<std::vector<float>> d_host(NL);
+        for (int j = 0; j < NL; ++j) {
+            bias[j] = j == 0 ? vb.p : hb[j - 1].p;
+            if (!base || !base[j]) continue;
+            const int w = width(j);
+            d_host[j].resize(w);
+            BM_CUDA(cudaMemcpyAsync(d_host[j].data(), bias[j], (size_t)w * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+            BM_CUDA(cudaStreamSynchronize(ctx->stream));
+            for (int c = 0; c < w; ++c) d_host[j][c] -= base[j][c];             // b_j - a_j in float32
+            a_dev[j].ensure(w); d_dev[j].ensure(w);
+            BM_CUDA(cudaMemcpyAsync(a_dev[j].p, base[j], (size_t)w * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+            BM_CUDA(cudaMemcpyAsync(d_dev[j].p, d_host[j].data(), (size_t)w * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+            abase[j] = a_dev[j].p; bias[j] = d_dev[j].p;
+        }
         std::vector<DevBuf<bf16_t>> buf(NL), buf2(NL);
         std::vector<bf16_t*> cur(NL), nxt(NL);
         for (int j = 0; j < NL; ++j) {
@@ -1543,9 +1569,9 @@ struct DbmTC : Dbm<float> {
             cur[j] = nxt[j] = buf[j].p;
             if (j % 2) { buf2[j].ensure((size_t)R * ldn[j]); buf2[j].zero(ctx->stream); nxt[j] = buf2[j].p; }
         }
-        for (int j = 1; j < NL; j += 2) {       // x_0 ~ Ber(1/2)   (:700-702)
+        for (int j = 1; j < NL; j += 2) {       // x_0 ~ Ber(1/2)   (:700-702), or Ber(sigmoid(a_j)): a_j broadcast to every run
             dim3 g(((width(j) + 3) / 4 + 127) / 128, R);
-            ais_unit_bf16_kernel<<<g, 128, 0, ctx->stream>>>(nullptr, 0, 0.f, cur[j], ldn[j], R, width(j), 1,
+            ais_unit_bf16_kernel<<<g, 128, 0, ctx->stream>>>(abase[j], 0, abase[j] ? 1.f : 0.f, cur[j], ldn[j], R, width(j), 1,
                                                              make_rng(seed, SITE_AIS_INIT, slot(j), 0, row0));
             count_launch(ctx);
         }
@@ -1567,14 +1593,13 @@ struct DbmTC : Dbm<float> {
             if (j == 0) {                                                 // x_1 W_0^T: W_0 stored [N, K]
                 g.A[0] = mat(x[1], R, Hs[0], ldn[1]); g.K[0] = Hs[0];
                 g.B[0] = mat(Wb[0].p, V, Hs[0], ldn[1]); g.b_t[0] = false;
-                g.bias = vb.p;
             } else {                                                      // x_{j-1} W_{j-1} (+ x_{j+1} W_j^T)
                 const int i = j - 1, in = width(j - 1);
                 g.A[0] = mat(x[j - 1], R, in, ldn[j - 1]); g.K[0] = in;
                 g.B[0] = mat(Wb[i].p, in, Hs[i], ldn[j]); g.b_t[0] = true;
                 if (j < L) above_pair(g, i, x[j + 1], R);
-                g.bias = hb[i].p;
             }
+            g.bias = bias[j]; g.ais_base = abase[j];
             dep0.push_back(j >= 1 ? last[j - 1] : -1); dep1.push_back(j + 1 < NL ? last[j + 1] : -1);
             return g;
         };

@@ -700,7 +700,8 @@ extern "C" int bm_debug_tc_op(bm_ctx* hctx, bm_tc_op_args* a) {
         vec[i].ensure((size_t)N);
         BM_CUDA(cudaMemcpyAsync(vec[i].p, vsrc[i], (size_t)N * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     }
-    g.bias = vec[0].p; g.sigma = vec[1].p; g.noise_sigma = vec[2].p;
+    g.bias = vec[0].p; g.sigma = vec[1].p;
+    if (a->ais_kind) g.ais_base = vec[2].p; else g.noise_sigma = vec[2].p;     // the AIS ops' base shares the slot
     g.acc_scale = a->acc_scale; g.bias_scale = a->bias_scale;
     g.act = a->act; g.sample = a->sample;
     g.rng = make_rng(a->seed, a->site, a->t, a->tick, a->row0);

@@ -82,6 +82,9 @@ constexpr int MAX_PHASES = 96;
 // (third-order series) relative to the term -- < 3e-6 and < 1e-8 for |z| <= 10 at these spacings, and both vanish with
 // sigma' for large |z|.  Coarser ladders take the closed form (MODE_AIS_UNITS_G).
 constexpr float AIS_MAX_CT = 2.5e-3f, AIS_MAX_CD = 4.0e-3f;
+// AIS ops run tiles of at most AIS_MAX_BN columns (fill_phase; tests may force wider ones without a base), so the upper half of
+// their shared bias slice holds the base bias a (x -log2 e) of the tile's columns
+constexpr int AIS_MAX_BN = 128;
 constexpr int SBIAS_BYTES = ACC_STAGES * MAX_BN * (int)sizeof(float);
 
 constexpr int SMEM_BYTES = RING_BYTES + OUT_BYTES + SMEM_BARRIER_BYTES + SBIAS_BYTES;     // 231,744 of 232,448
@@ -400,6 +403,7 @@ struct EpiCtx {
     int n_blk, split;             // the tile's column block and K split
     int lane;
     const float* sbias;           // shared memory: bias_scale * bias (x -log2 e for sigmoid) of the tile's columns
+    bool base;                    // AIS: sbias[AIS_MAX_BN ..] holds the base a x -log2 e of the tile's columns
     uint32_t out_base;            // shared address of the staging FIFO
     uint64_t* out_full;           // [N_OUT_BUF] a staged granule is complete (8 warp arrivals)
     uint64_t* out_free;           // [N_OUT_BUF] its TMA store has read the buffer (publisher)
@@ -407,10 +411,11 @@ struct EpiCtx {
     uint32_t mant_mask, one_bits; // TcLaunch::mant_mask / one_bits
 };
 
-// softplus(b z) - softplus(a z) = log1p(sigmoid(a z) * expm1((b - a) z)) without cancellation (b - a ~ 1e-3): short series
-// where both arguments are small (the common case), the library functions elsewhere
-__device__ __forceinline__ float ais_softplus_diff(float a, float b, float z) {
-    const float sa = sigmoid_from_neg_log2(a * z * -1.4426950408889634f);
+// softplus(b z + a0) - softplus(a z + a0) = log1p(sigmoid(a z + a0) * expm1((b - a) z)) without cancellation (b - a ~ 1e-3):
+// short series where both arguments are small (the common case), the library functions elsewhere.  aq = a0 * -log2 e is the
+// AIS base of the column (0: no base)
+__device__ __forceinline__ float ais_softplus_diff(float a, float b, float z, float aq) {
+    const float sa = sigmoid_from_neg_log2(fmaf(a * z, -1.4426950408889634f, aq));
     const float t = (b - a) * z;
     float em;
     if (fabsf(t) < 0.03f) em = t * fmaf(t, fmaf(t, fmaf(t, fmaf(t, 1.0f / 120.0f, 1.0f / 24.0f), 1.0f / 6.0f), 0.5f), 1.0f);
@@ -423,10 +428,11 @@ __device__ __forceinline__ float ais_softplus_diff(float a, float b, float z) {
 // Two adjacent accumulator columns (n, n + 1; n even) of one row m: activation, sampling, packed bf16 mean / state and the
 // fp32 store.  wf / ws are the Philox words of the two columns: words 2 (n % 4 / 2) and 2 (n % 4 / 2) + 1 of the row's
 // block n / 4 -- the same draws, column for column, as a thread that owns the whole block.
-// Returns the pair's contribution to the row's AIS log-weight (AIS modes) or 0.
+// Returns the pair's contribution to the row's AIS log-weight (AIS modes) or 0.  aq0 / aq1: the AIS base of the two columns
+// (x -log2 e; 0 without a base), added to every sigmoid argument after the beta scaling.
 template <int MODE>
 __device__ __forceinline__ float pair_body(const EpiCtx& c, float v0, float v1, uint32_t wf, uint32_t ws, float b0, float b1,
-                                           int n, int m, bool row_ok, float* out_f32, bool f32_vec,
+                                           float aq0, float aq1, int n, int m, bool row_ok, float* out_f32, bool f32_vec,
                                            uint32_t& mean_pk, uint32_t& state_pk) {
     typedef EpiCfg<MODE> E;
     const EpiPhase& p = c.p;
@@ -440,6 +446,7 @@ __device__ __forceinline__ float pair_body(const EpiCtx& c, float v0, float v1, 
     const bool do_f32 = E::fixed ? E::f32 : (out_f32 != nullptr);
     const float v[2] = {v0, v1};
     const float bq[2] = {b0, b1};
+    const float aq[2] = {aq0, aq1};
     const uint32_t words[2] = {wf, ws};
     float g[2] = {0.f, 0.f};
     if (!E::fixed && smp == SMP_GAUSSIAN) {
@@ -464,7 +471,7 @@ __device__ __forceinline__ float pair_body(const EpiCtx& c, float v0, float v1, 
             //   with t = (b - a) z, m = (a + b) / 2, and sigmoid(m z) = sigmoid(beta_next z - d), d = (beta_next - m) z, as its
             //   third-order series in d around p (error terms: AIS_MAX_CT / AIS_MAX_CD above).
             float e_, p_;
-            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e_) : "f"(x * p.ais_next * -1.4426950408889634f));
+            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e_) : "f"(fmaf(x * p.ais_next, -1.4426950408889634f, aq[j])));
             asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(p_) : "f"(1.0f + e_));
             s_ = ((u32_to_one_two(words[j], c.mant_mask, c.one_bits) - 1.0f) < p_) ? 1.0f : 0.0f;
             if (MODE == MODE_AIS_UNITS) {
@@ -481,9 +488,9 @@ __device__ __forceinline__ float pair_body(const EpiCtx& c, float v0, float v1, 
         }
         if (MODE == MODE_AIS_UNITS_G) {
             // any temperatures, optional sampling / output: the closed forms
-            if (p.ais_logw && valid) ais_part += ais_softplus_diff(p.ais_a, p.ais_b, x);
+            if (p.ais_logw && valid) ais_part += ais_softplus_diff(p.ais_a, p.ais_b, x, aq[j]);
             float e_;
-            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e_) : "f"(x * p.ais_next * -1.4426950408889634f));
+            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e_) : "f"(fmaf(x * p.ais_next, -1.4426950408889634f, aq[j])));
             const float d_ = 1.0f + e_;
             if (smp == SMP_BERNOULLI) {
                 const float u12 = u32_to_one_two(words[j], c.mant_mask, c.one_bits);
@@ -498,7 +505,7 @@ __device__ __forceinline__ float pair_body(const EpiCtx& c, float v0, float v1, 
             // only the draw is needed: u < 1/(1+e)  <=>  u*(1+e) < 1, with u = u12 - 1 folded into one FMA
             // (no reciprocal, no "- 1.0f"); e = inf (p = 0) gives NaN -> 0, e = 0 (p = 1) gives u < 1 -> 1
             float e_;
-            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e_) : "f"(x));
+            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e_) : "f"(MODE == MODE_AIS_STATE ? x + aq[j] : x));
             const float d_ = 1.0f + e_;
             const float u12 = u32_to_one_two(words[j], c.mant_mask, c.one_bits);
             s_ = (fmaf(u12, d_, -d_) < 1.0f) ? 1.0f : 0.0f;
@@ -595,9 +602,10 @@ __device__ __forceinline__ void epilogue_tile(const EpiCtx& c, const float (&acc
                     else { w0f = got_f; w0s = got_s; w1f = w.z; w1s = w.w; }
                 }
                 const float2 b2 = *reinterpret_cast<const float2*>(c.sbias + j * GRAN_COLS + cl);
+                const float2 a2 = (E::ais && c.base) ? *reinterpret_cast<const float2*>(c.sbias + AIS_MAX_BN + j * GRAN_COLS + cl) : make_float2(0.f, 0.f);
                 uint32_t mp0, sp0, mp1, sp1;
-                ais0 += pair_body<MODE>(c, acc_at(acc, j, 4 * i), acc_at(acc, j, 4 * i + 1), w0f, w0s, b2.x, b2.y, n, c.m0, ok0, out_f32, f32_vec, mp0, sp0);
-                ais1 += pair_body<MODE>(c, acc_at(acc, j, 4 * i + 2), acc_at(acc, j, 4 * i + 3), w1f, w1s, b2.x, b2.y, n, m1, ok1, out_f32, f32_vec, mp1, sp1);
+                ais0 += pair_body<MODE>(c, acc_at(acc, j, 4 * i), acc_at(acc, j, 4 * i + 1), w0f, w0s, b2.x, b2.y, a2.x, a2.y, n, c.m0, ok0, out_f32, f32_vec, mp0, sp0);
+                ais1 += pair_body<MODE>(c, acc_at(acc, j, 4 * i + 2), acc_at(acc, j, 4 * i + 3), w1f, w1s, b2.x, b2.y, a2.x, a2.y, n, m1, ok1, out_f32, f32_vec, mp1, sp1);
                 // columns past N and rows past M are written to the staging buffer too: the TMA store clips them
                 const uint32_t u = (((uint32_t)i ^ swz) << 4);
                 if (do_mean) { sts32(smem_mean + off0 + u, mp0); sts32(smem_mean + off1 + u, mp1); }
@@ -891,8 +899,14 @@ tc_program_kernel(const __grid_constant__ TcLaunch L) {
                 const float bsc = (ph->act == ACT_SIGMOID) ? ph->bias_scale * -1.4426950408889634f : ph->bias_scale;
                 const int n = u.n_blk * ph->BN + et;
                 if (et < MAX_BN) s_bias[acc_st * MAX_BN + et] = (ph->bias && et < ph->BN && n < ph->N) ? bsc * __ldg(ph->bias + n) : 0.f;
+                const bool base = ph->ais_kind && ph->ais_base;     // AIS: the base of the tile's columns (BN <= AIS_MAX_BN)
+                if (base && et >= AIS_MAX_BN) {
+                    const int nb = n - AIS_MAX_BN;
+                    s_bias[acc_st * MAX_BN + et] = (et - AIS_MAX_BN < ph->BN && nb < ph->N) ? -1.4426950408889634f * __ldg(ph->ais_base + nb) : 0.f;
+                }
                 asm volatile("bar.sync 1, 256;" ::: "memory");
                 c.sbias = s_bias + acc_st * MAX_BN;
+                c.base = base;
             }
             // ---- mainloop: one wgmma group per K chunk, the previous chunk's stage released once its group retired
             const int bn16 = ph->BN / 16;
@@ -1063,10 +1077,12 @@ static void fill_phase(Ctx* ctx, const TcGemm& g, int cluster, TcPhase& ph) {
     const int nsplit = g.splits > 0 ? g.splits : 1;
     // AIS ops stay at 128 columns or less: their epilogues (a softplus difference or a series per element, an fp64 atomic per
     // row and tile) cost more than the model's per-column term, and an AIS ladder of the cfg4 DBM measured 7% slower at 256
-    const int max_bn = g.ais_kind ? 128 : MAX_BN;
+    const int max_bn = g.ais_kind ? AIS_MAX_BN : MAX_BN;
     TilePick tp = pick_tile(g.N, m_tiles, nsplit, (chunks_total + nsplit - 1) / nsplit, ctx->sm_count, cluster, max_bn);
     if (g.force_bn > 0) tp.bn = g.force_bn;
     BM_REQUIRE(tp.cluster == cluster, "tile picker returned another row grouping");
+    BM_REQUIRE(!g.ais_base || tp.bn <= AIS_MAX_BN, "AIS ops with a base run tiles of at most 128 columns");
+    BM_REQUIRE(!g.ais_base || g.ais_kind, "a base bias belongs to an AIS op");
     bool b_mn = false;
     for (int i = 0; i < g.n_pairs; ++i) b_mn = b_mn || g.b_t[i];
     const bool staged_out = g.out_mean_bf != nullptr || g.out_state_bf != nullptr;
@@ -1093,6 +1109,7 @@ static void fill_phase(Ctx* ctx, const TcGemm& g, int cluster, TcPhase& ph) {
     BM_REQUIRE(p.splits == 1 || (g.out_f32 && !g.out_mean_bf && !g.out_state_bf), "split-K writes fp32 partials only");
     p.acc_scale = g.acc_scale; p.bias_scale = g.bias_scale;
     p.bias = g.bias; p.sigma = g.sigma; p.noise_sigma = g.noise_sigma;
+    if (g.ais_kind) p.ais_base = g.ais_base;          // AIS ops have no noise_sigma (required below)
     p.act = g.act; p.sample = g.sample; p.mode = epilogue_mode(g);
     p.k0 = g.rng.k0; p.k1 = g.rng.k1;
     p.rng_c2 = g.rng.c2;

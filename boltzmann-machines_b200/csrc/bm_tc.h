@@ -62,6 +62,7 @@ struct TcGemm {
     int ais_kind = 0;
     float ais_a = 0.f, ais_b = 0.f, ais_next = 0.f, ais_lin = 0.f;
     double* ais_logw = nullptr;
+    const float* ais_base = nullptr;  // AIS ops: per-column base bias a, + a after the beta scaling (TcPhaseLite::ais_base)
     uint32_t tick_off = 0;
     uint32_t row_off = 0;             // draws of row r come from row rng.row0 + row_off + r (slot m of a tempered ladder: m * rows)
 };

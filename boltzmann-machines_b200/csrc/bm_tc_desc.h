@@ -22,7 +22,11 @@ struct TcPhaseLite {
     float acc_scale, bias_scale;
     const float* bias;
     const float* sigma;
-    const float* noise_sigma;
+    union {
+        const float* noise_sigma;    // Gaussian draws
+        const float* ais_base;       // AIS ops (which never draw Gaussians): per-column base bias a, added after the beta
+                                     // scaling -- sigmoid(beta u + a) (DESIGN.md §5.4d); nullable, null is a = 0
+    };
     int act, sample, mode;
     uint32_t k0, k1;                 // Philox key of this op's draws (an engine's own programs: the launch key; training groups:
                                      // each member's seed)
@@ -48,6 +52,9 @@ struct TcPhaseLite {
     // skipped when ais_logw is null) and, if a state output is given, emits sample(sigmoid(ais_next * z)) -- the unit updates of the
     // next transition.  ais_kind 2 ("state"): an ordinary sigmoid / Bernoulli op whose epilogue also adds
     // ais_lin * sum_n state[n] * (bias_scale * bias[n] * -log2 e)  to ais_logw[row]  (the linear term of log p*, dbm.py:658).
+    // With a base (ais_base above) every sigmoid argument gains + a[n]: the units op draws from sigmoid(ais_next z + a) and adds
+    // softplus(ais_b z + a) - softplus(ais_a z + a); the state op draws from sigmoid(acc_scale acc + bias_scale bias + a), and
+    // its linear term stays without a.
     int ais_kind;
     float ais_a, ais_b, ais_next, ais_lin;
     double* ais_logw;

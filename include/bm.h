@@ -281,6 +281,20 @@ int  bm_dbm_ais(bm_dbm* dbm, int32_t n_runs, int32_t n_betas, int32_t n_gibbs_st
  * themselves (one process driving several GPUs; more runs than fit in memory at once) */
 int  bm_dbm_ais_rows(bm_dbm* dbm, int32_t n_runs, int32_t n_betas, int32_t n_gibbs_steps, uint64_t seed, uint32_t first_run,
                      double* logZ);
+/* AIS from a base-rate model (DESIGN.md §5.4d; Salakhutdinov & Hinton 2009): the ladder starts from the factorial model
+ * p_A(x) ∝ exp(sum_j a_j.x_j) over every unit layer instead of the uniform one, along p_beta ∝ p_A^(1-beta) p^beta (weights
+ * scaled by beta, layer j's bias beta b_j + (1 - beta) a_j), and each run's estimate includes
+ * log Z_A = sum_j sum_n softplus(a_{j,n}) (float64).  base is NULL or n_hiddens + 1 host pointers (v, h_1 .. h_L), each NULL
+ * (a_j = 0) or [width of layer j] floats; a typical base sets a_v to the log-odds of the training data's pixel means and leaves
+ * the hidden layers NULL.  NULL or all-NULL is bm_dbm_ais / bm_dbm_ais_rows exactly (those two call these).  With any base the
+ * ladder runs over the odd layers at every depth, 2 included, and the run keys are those of bm_dbm_ais, so sharded, sliced and
+ * single calls agree.  Refused before any launch: BM_EINVAL for a non-finite base entry; BM_EUNSUPPORTED on the CUDA-core engine
+ * (float64 models, BM_COMPUTE_FP32), for Gaussian visibles or multinomial layers, an odd layer h_1, h_3, ... that is not
+ * sampled, and for classification DBMs. */
+int  bm_dbm_ais_base(bm_dbm* dbm, int32_t n_runs, int32_t n_betas, int32_t n_gibbs_steps, uint64_t seed, const float* const* base,
+                     double* logZ);
+int  bm_dbm_ais_base_rows(bm_dbm* dbm, int32_t n_runs, int32_t n_betas, int32_t n_gibbs_steps, uint64_t seed, uint32_t first_run,
+                          const float* const* base, double* logZ);
 /* parallel tempering: swaps accepted / proposed between slots m and m+1 since create, n_temps-1 entries each (BM_EINVAL
  * without tempering) */
 int  bm_dbm_pt_counts(bm_dbm* dbm, int64_t* accepted, int64_t* proposed);
@@ -335,7 +349,7 @@ typedef struct bm_tc_op_args {
     float acc_scale, bias_scale;
     const float* bias;                     /* [N] or NULL (host) */
     const float* sigma;                    /* [N] or NULL */
-    const float* noise_sigma;              /* [N] or NULL */
+    const float* noise_sigma;              /* [N] or NULL; an AIS op (ais_kind != 0) reads it as its base bias a (DESIGN.md §5.4d) */
     int32_t act, sample;                   /* 0 linear, 1 sigmoid, 2 softplus;  0 none, 1 Bernoulli, 2 Gaussian */
     uint64_t seed;
     uint32_t site, t, tick, row0, tick_off;
