@@ -31,7 +31,7 @@ EXPORTS = (
     'bm_dbm_create', 'bm_dbm_destroy', 'bm_dbm_set_param', 'bm_dbm_get_param', 'bm_dbm_init_particles',
     'bm_dbm_train_step', 'bm_dbm_val_metrics', 'bm_dbm_transform', 'bm_dbm_reconstruct', 'bm_dbm_log_proba',
     'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows', 'bm_dbm_ais_base', 'bm_dbm_ais_base_rows', 'bm_dbm_pt_counts', 'bm_debug_dbm_multinomial_rows',
-    'bm_dbm_train_step_labeled', 'bm_dbm_predict_proba', 'bm_dbm_fill', 'bm_dbm_debug_last_fill',
+    'bm_dbm_train_step_labeled', 'bm_dbm_predict_proba', 'bm_dbm_fill', 'bm_dbm_debug_last_fill', 'bm_dbm_debug_last_sample_v',
     'bm_crbm_create', 'bm_crbm_destroy', 'bm_crbm_set_param', 'bm_crbm_get_param', 'bm_crbm_init_weights',
     'bm_crbm_train_step', 'bm_crbm_predict_proba', 'bm_crbm_transform', 'bm_crbm_debug_last_step',
     'bm_rbm_group_create', 'bm_rbm_group_destroy', 'bm_rbm_group_train_epoch', 'bm_rbm_group_train_epoch_u8',
@@ -172,6 +172,7 @@ def load_library(path=None):
         'bm_dbm_predict_proba': [vp, vp, i32, vp],
         'bm_dbm_fill': [vp, vp, vp, vp, i32, u32, i32, u64, u32, vp],
         'bm_dbm_debug_last_fill': [vp, C.c_char_p, vp, sz],
+        'bm_dbm_debug_last_sample_v': [vp, C.c_char_p, vp, sz],
         'bm_debug_dbm_multinomial_rows': [vp, vp, i32, i32, dbl, i32, u64, u32, u32, u32, vp, vp, vp, vp],
         'bm_crbm_create': [vp, C.POINTER(CrbmCfg), C.POINTER(vp)],
         'bm_crbm_set_param': [vp, C.c_char_p, vp, sz], 'bm_crbm_get_param': [vp, C.c_char_p, vp, sz],
@@ -961,6 +962,18 @@ class CudaDBM(object):
         tc = self.compute == 'bf16' and self.dt == np.float32 and self._is_tc()
         a = np.empty((int(rows), width), dtype=np.uint16 if tc else self.dt)
         check(self._lib.bm_dbm_debug_last_fill(self.handle, name.encode(), a.ctypes.data, a.nbytes))
+        return (a.astype(np.uint32) << 16).view(np.float32) if tc else a
+
+    def debug_last_sample_v(self, name):
+        """one sweep of the last ``sample_v``'s uncommitted half (include/bm.h bm_dbm_debug_last_sample_v): "v", "h", "h_1", ...
+        for its last sweep, + "_prev" for the sweep before; [n_particles, n], float32 widened from bf16 on the tensor-core
+        engine, the model dtype on the CUDA-core engine"""
+        base = name[:-5] if name.endswith('_prev') else name
+        sizes = {'v': self.V}
+        sizes.update({'h' + _sfx(i): self.Hs[i] for i in range(self.L)})
+        tc = self.compute == 'bf16' and self.dt == np.float32 and self._is_tc()
+        a = np.empty((self.M, sizes[base]), dtype=np.uint16 if tc else self.dt)
+        check(self._lib.bm_dbm_debug_last_sample_v(self.handle, name.encode(), a.ctypes.data, a.nbytes))
         return (a.astype(np.uint32) << 16).view(np.float32) if tc else a
 
     def _is_tc(self):

@@ -265,6 +265,7 @@ struct DbmBase {
     virtual void fill(const void* X, const uint8_t* mask, const int32_t* labels, int rows, uint32_t row0, int k, uint64_t seed,
                       uint32_t tick, void* out) = 0;
     virtual void fill_debug(const char* name, void* host, size_t bytes) = 0;
+    virtual void sample_v_debug(const char* name, void* host, size_t bytes) = 0;
 };
 
 // Parallel tempering (bm_dbm_cfg.n_temps / betas): what the engines refuse before anything is allocated.  0 / NULL is off.
@@ -540,6 +541,7 @@ struct Dbm : DbmBase {
 
     // ---- PCD particle update (dbm.py:480-509) --------------------------------------------------------------
     void particles_update(int n_steps, bool sample, uint64_t seed, uint32_t tick, int t0, bool commit, T** v_final) {
+        sv_k = 0;                                     // h2 / v2 are about to be overwritten: no sample_v chain to report
         std::vector<T*> cur(L), nxt(L), spare(L);
         for (int i = 0; i < L; ++i) { cur[i] = h[i].p; nxt[i] = h2[i].p; spare[i] = nullptr; }
         T* vc = v.p; T* vn = v2.p; T* vspare = nullptr;
@@ -659,6 +661,30 @@ struct Dbm : DbmBase {
         particles_update(k, false, seed, tick, k, false, &vf);
         if (vf != v.p) BM_CUDA(cudaMemcpyAsync(v.p, vf, (size_t)M * V * sizeof(T), cudaMemcpyDeviceToDevice, ctx->stream));
         BM_CUDA(cudaMemcpyAsync(out, v.p, (size_t)M * V * sizeof(T), cudaMemcpyDeviceToHost, ctx->stream));
+        BM_CUDA(cudaStreamSynchronize(ctx->stream));
+        sv_k = k;
+    }
+    // The uncommitted sweeps of the last sample_v ping-pong on scratch: sweep t (1..k) is in h2 / v2 for odd t, h3 / v3 for even
+    // t, untouched until the next particle update.  "v", "h", "h_1", ...: sweep k; + "_prev": sweep k - 1 (k >= 2).  [M, n].
+    int sv_k = 0;                                 // sweeps of the last sample_v's uncommitted run (0: none to report)
+    void sample_v_debug(const char* name, void* host, size_t bytes) override {
+        BM_REQUIRE(sv_k > 0, "sample_v_debug: no uncommitted sample_v sweep since the last particle update");
+        std::string n(name);
+        int t = sv_k;
+        const std::string suffix = "_prev";
+        if (n.size() > suffix.size() && n.compare(n.size() - suffix.size(), suffix.size(), suffix) == 0) {
+            n = n.substr(0, n.size() - suffix.size()); --t;
+        }
+        BM_REQUIRE(t >= 1, "sample_v_debug: the sweep before the first uncommitted one is the committed particles (get_param)");
+        const bool odd = (t & 1) != 0;
+        const T* src = nullptr; int width = 0;
+        if (n == "v") { src = odd ? v2.p : v3.p; width = V; }
+        else
+            for (int i = 0; i < L; ++i)
+                if (n == "h" + sfx(i)) { src = odd ? h2[i].p : h3[i].p; width = Hs[i]; }
+        BM_REQUIRE(src, std::string("sample_v_debug: unknown name '") + name + "'");
+        BM_REQUIRE(bytes == (size_t)M * width * sizeof(T), std::string("sample_v_debug: size mismatch for '") + name + "'");
+        BM_CUDA(cudaMemcpyAsync(host, src, bytes, cudaMemcpyDeviceToHost, ctx->stream));
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
     }
 
@@ -963,6 +989,9 @@ int bm_dbm_fill(bm_dbm* h, const void* X, const uint8_t* mask, const int32_t* la
 }
 int bm_dbm_debug_last_fill(bm_dbm* h, const char* name, void* host, size_t bytes) {
     BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(name && host, "null argument"); DBM(h)->fill_debug(name, host, bytes); BM_API_END
+}
+int bm_dbm_debug_last_sample_v(bm_dbm* h, const char* name, void* host, size_t bytes) {
+    BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(name && host, "null argument"); DBM(h)->sample_v_debug(name, host, bytes); BM_API_END
 }
 
 int bm_debug_dbm_multinomial_rows(bm_ctx* hctx, const float* pre, int32_t rows, int32_t cols, double n_samples, int32_t n_draws,

@@ -1059,6 +1059,7 @@ struct DbmTC : Dbm<float> {
     // longer chains take one launch per op.  With tempering, a committed update runs every slot (cut into launches between
     // sweeps when it is long) and ends with a swap round; an uncommitted run only needs slot 0, whose output it is.
     void particles_tc(int n_steps, bool sample, uint64_t seed, uint32_t tick, int t0, bool commit, bf16_t** v_final) {
+        sv_k = 0;                                     // h2_b / v2_b are about to be overwritten
         if (commit && T > 1) {
             if (n_steps >= 1) particles_program_pt(n_steps, sample, seed, tick, t0);
             pt_swap_round(seed, tick);
@@ -1304,6 +1305,30 @@ struct DbmTC : Dbm<float> {
         particles_f32_stale = true;
         widen_particles();
         BM_CUDA(cudaMemcpyAsync(out, v.p, (size_t)M * V * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+        BM_CUDA(cudaStreamSynchronize(ctx->stream));
+        sv_k = k;
+    }
+    // as Dbm<T>::sample_v_debug on the bf16 ping-pong (h2_b / v2_b for odd sweeps, h3_b / v3_b for even ones; slot 0's rows),
+    // as bf16 bit patterns
+    void sample_v_debug(const char* name, void* host, size_t bytes) override {
+        BM_REQUIRE(sv_k > 0, "sample_v_debug: no uncommitted sample_v sweep since the last particle update");
+        std::string n(name);
+        int t = sv_k;
+        const std::string suffix = "_prev";
+        if (n.size() > suffix.size() && n.compare(n.size() - suffix.size(), suffix.size(), suffix) == 0) {
+            n = n.substr(0, n.size() - suffix.size()); --t;
+        }
+        BM_REQUIRE(t >= 1, "sample_v_debug: the sweep before the first uncommitted one is the committed particles (get_param)");
+        const bool odd = (t & 1) != 0;
+        const bf16_t* src = nullptr; int width = 0, ld = 0;
+        if (n == "v") { src = odd ? v2_b.p : v3_b.p; width = V; ld = ldn[0]; }
+        else
+            for (int i = 0; i < L; ++i)
+                if (n == "h" + sfx(i)) { src = odd ? h2_b[i].p : h3_b[i].p; width = Hs[i]; ld = ldn[i + 1]; }
+        BM_REQUIRE(src, std::string("sample_v_debug: unknown name '") + name + "'");
+        BM_REQUIRE(bytes == (size_t)M * width * sizeof(bf16_t), std::string("sample_v_debug: size mismatch for '") + name + "'");
+        BM_CUDA(cudaMemcpy2DAsync(host, (size_t)width * sizeof(bf16_t), src, (size_t)ld * sizeof(bf16_t), (size_t)width * sizeof(bf16_t),
+                                  M, cudaMemcpyDeviceToHost, ctx->stream));
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
     }
 

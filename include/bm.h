@@ -317,6 +317,13 @@ int  bm_dbm_fill(bm_dbm* dbm, const void* X, const uint8_t* mask, const int32_t*
  * the tensor-core engine, the model dtype on the CUDA-core engine.  Device-to-host copies only.  BM_EINVAL for an unknown name,
  * a wrong size, or before the first fill. */
 int  bm_dbm_debug_last_fill(bm_dbm* dbm, const char* name, void* host, size_t bytes);
+/* test hook: one sweep of the uncommitted second half of the last bm_dbm_sample_v, [n_particles, n] row-major without padding
+ * (slot 0's particles on a tempered DBM).  "v", "h", "h_1", ...: the visible / hidden means of its last sweep (k); the same
+ * names + "_prev": of sweep k - 1 (k >= 2; sweep 0 is the committed particles, read with bm_dbm_get_param).  Elements: bf16 bit
+ * patterns (uint16) on the tensor-core engine, the model dtype on the CUDA-core engine.  Reads the scratch the sweeps ran on;
+ * a device-to-host copy only, no launch.  BM_EINVAL for an unknown name, a wrong size, after k = 0, or once any particle update
+ * has run since. */
+int  bm_dbm_debug_last_sample_v(bm_dbm* dbm, const char* name, void* host, size_t bytes);
 
 /* ---- test hook: the raw tensor-core GEMM (no counterpart in the reference) -----------------
  * C[M,N] (fp32) = A * B^T (+/- A2 * B2^T), operands given as host fp32 and rounded to bf16.
