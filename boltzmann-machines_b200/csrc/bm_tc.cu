@@ -16,8 +16,8 @@
 //
 // Per CTA (384 threads, one CTA per SM, 128-row tiles; a "pair" is two CTAs that own the two
 // 128-row blocks of a 256-row group -- a scheduling unit of the dataflow, the CTAs share nothing):
-//   warps 0-7  two consumer warpgroups: warpgroup g issues wgmma m64n64k16 for tile rows 64g..64g+63
-//              (one instruction per 64-column block of the tile and one for a last 16/32/48-column block, accumulators in registers), then runs
+//   warps 0-7  two consumer warpgroups: warpgroup g issues wgmma m64nNk16 for tile rows 64g..64g+63
+//              (one instruction across the tile's whole width N = BN per K=16 step, accumulators in registers), then runs
 //              the epilogue on its accumulators: bias, sigmoid by ex2/rcp, Philox-4x32-10 in registers,
 //              bf16 outputs into a 128B-swizzled staging FIFO, fp32 outputs straight to global memory
 //   warp 11    TMA producer: 128B-swizzled tiles, mbarrier ring of 3 x 48 KiB (BN = 256) to 6 x 24 KiB (BN = 64) stages
@@ -204,67 +204,55 @@ __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.alig
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// D[64xN] (+)= (+/-A)[64x16] * B[16xN], N = 16, 32, 48 or 64: bf16 operands from shared memory, fp32 accumulator fragment `d`
-// (thread t of the warpgroup holds rows 16 (t/32) + (t%32)/4 (+8) and columns 8 i + 2 (t%4) (+1), registers 4 i .. 4 i + 3).
-// TA / TB: the operand is MN-major (wgmma transpose bit); NEG: scale-a = -1.
-template <int TA, int TB, int NEG>
-__device__ __forceinline__ void wgmma_n16(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %10, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7}, "
-        "%8, %9, p, %11, 1, %12, %13;\n\t"
-        "}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-        : "l"(da), "l"(db), "r"(scale_d), "n"(NEG ? -1 : 1), "n"(TA), "n"(TB));
-}
-template <int TA, int TB, int NEG>
-__device__ __forceinline__ void wgmma_n32(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %18, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-        "%16, %17, p, %19, 1, %20, %21;\n\t"
-        "}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "l"(da), "l"(db), "r"(scale_d), "n"(NEG ? -1 : 1), "n"(TA), "n"(TB));
-}
-template <int TA, int TB, int NEG>
-__device__ __forceinline__ void wgmma_n48(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %26, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, "
-        "%24, %25, p, %27, 1, %28, %29;\n\t"
-        "}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-        : "l"(da), "l"(db), "r"(scale_d), "n"(NEG ? -1 : 1), "n"(TA), "n"(TB));
-}
-template <int TA, int TB, int NEG>
-__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-        "%32, %33, p, %35, 1, %36, %37;\n\t"
-        "}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "l"(da), "l"(db), "r"(scale_d), "n"(NEG ? -1 : 1), "n"(TA), "n"(TB));
-}
-template <int N, int TA, int TB, int NEG>
-__device__ __forceinline__ void wgmma_m64nk16(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
-    if constexpr (N == 16) wgmma_n16<TA, TB, NEG>(d, da, db, scale_d);
-    else if constexpr (N == 32) wgmma_n32<TA, TB, NEG>(d, da, db, scale_d);
-    else if constexpr (N == 48) wgmma_n48<TA, TB, NEG>(d, da, db, scale_d);
-    else wgmma_n64<TA, TB, NEG>(d, da, db, scale_d);
+// D[64 x 16 BN16] (+)= (+/-A)[64x16] * B[16 x 16 BN16]: one wgmma.m64nNk16 over the first 8 BN16 accumulator registers (bf16
+// operands from shared memory, fp32 accumulator fragment `d`; thread t of the warpgroup holds rows 16 (t/32) + (t%32)/4 (+8) and
+// columns 8 i + 2 (t%4) (+1) in registers 4 i .. 4 i + 3, i.e. 64-column block j in d[j]).  TA / TB: the operand is MN-major
+// (wgmma transpose bit); NEG: scale-a = -1.  Every shape names all 128 accumulator registers as operands, so the inputs keep
+// their operand numbers and one asm statement serves every width; the registers past 8 BN16 are not touched.
+#define BM_WG_REGS_1 "%0, %1, %2, %3, %4, %5, %6, %7"
+#define BM_WG_REGS_2 BM_WG_REGS_1 ", %8, %9, %10, %11, %12, %13, %14, %15"
+#define BM_WG_REGS_3 BM_WG_REGS_2 ", %16, %17, %18, %19, %20, %21, %22, %23"
+#define BM_WG_REGS_4 BM_WG_REGS_3 ", %24, %25, %26, %27, %28, %29, %30, %31"
+#define BM_WG_REGS_5 BM_WG_REGS_4 ", %32, %33, %34, %35, %36, %37, %38, %39"
+#define BM_WG_REGS_6 BM_WG_REGS_5 ", %40, %41, %42, %43, %44, %45, %46, %47"
+#define BM_WG_REGS_7 BM_WG_REGS_6 ", %48, %49, %50, %51, %52, %53, %54, %55"
+#define BM_WG_REGS_8 BM_WG_REGS_7 ", %56, %57, %58, %59, %60, %61, %62, %63"
+#define BM_WG_REGS_9 BM_WG_REGS_8 ", %64, %65, %66, %67, %68, %69, %70, %71"
+#define BM_WG_REGS_10 BM_WG_REGS_9 ", %72, %73, %74, %75, %76, %77, %78, %79"
+#define BM_WG_REGS_11 BM_WG_REGS_10 ", %80, %81, %82, %83, %84, %85, %86, %87"
+#define BM_WG_REGS_12 BM_WG_REGS_11 ", %88, %89, %90, %91, %92, %93, %94, %95"
+#define BM_WG_REGS_13 BM_WG_REGS_12 ", %96, %97, %98, %99, %100, %101, %102, %103"
+#define BM_WG_REGS_14 BM_WG_REGS_13 ", %104, %105, %106, %107, %108, %109, %110, %111"
+#define BM_WG_REGS_15 BM_WG_REGS_14 ", %112, %113, %114, %115, %116, %117, %118, %119"
+#define BM_WG_REGS_16 BM_WG_REGS_15 ", %120, %121, %122, %123, %124, %125, %126, %127"
+#define BM_WG_ACC \
+    "+f"(d[0][0]), "+f"(d[0][1]), "+f"(d[0][2]), "+f"(d[0][3]), "+f"(d[0][4]), "+f"(d[0][5]), "+f"(d[0][6]), "+f"(d[0][7]), "+f"(d[0][8]), "+f"(d[0][9]), "+f"(d[0][10]), "+f"(d[0][11]), "+f"(d[0][12]), "+f"(d[0][13]), "+f"(d[0][14]), "+f"(d[0][15]), "+f"(d[0][16]), "+f"(d[0][17]), "+f"(d[0][18]), "+f"(d[0][19]), "+f"(d[0][20]), "+f"(d[0][21]), "+f"(d[0][22]), "+f"(d[0][23]), "+f"(d[0][24]), "+f"(d[0][25]), "+f"(d[0][26]), "+f"(d[0][27]), "+f"(d[0][28]), "+f"(d[0][29]), "+f"(d[0][30]), "+f"(d[0][31]), \
+    "+f"(d[1][0]), "+f"(d[1][1]), "+f"(d[1][2]), "+f"(d[1][3]), "+f"(d[1][4]), "+f"(d[1][5]), "+f"(d[1][6]), "+f"(d[1][7]), "+f"(d[1][8]), "+f"(d[1][9]), "+f"(d[1][10]), "+f"(d[1][11]), "+f"(d[1][12]), "+f"(d[1][13]), "+f"(d[1][14]), "+f"(d[1][15]), "+f"(d[1][16]), "+f"(d[1][17]), "+f"(d[1][18]), "+f"(d[1][19]), "+f"(d[1][20]), "+f"(d[1][21]), "+f"(d[1][22]), "+f"(d[1][23]), "+f"(d[1][24]), "+f"(d[1][25]), "+f"(d[1][26]), "+f"(d[1][27]), "+f"(d[1][28]), "+f"(d[1][29]), "+f"(d[1][30]), "+f"(d[1][31]), \
+    "+f"(d[2][0]), "+f"(d[2][1]), "+f"(d[2][2]), "+f"(d[2][3]), "+f"(d[2][4]), "+f"(d[2][5]), "+f"(d[2][6]), "+f"(d[2][7]), "+f"(d[2][8]), "+f"(d[2][9]), "+f"(d[2][10]), "+f"(d[2][11]), "+f"(d[2][12]), "+f"(d[2][13]), "+f"(d[2][14]), "+f"(d[2][15]), "+f"(d[2][16]), "+f"(d[2][17]), "+f"(d[2][18]), "+f"(d[2][19]), "+f"(d[2][20]), "+f"(d[2][21]), "+f"(d[2][22]), "+f"(d[2][23]), "+f"(d[2][24]), "+f"(d[2][25]), "+f"(d[2][26]), "+f"(d[2][27]), "+f"(d[2][28]), "+f"(d[2][29]), "+f"(d[2][30]), "+f"(d[2][31]), \
+    "+f"(d[3][0]), "+f"(d[3][1]), "+f"(d[3][2]), "+f"(d[3][3]), "+f"(d[3][4]), "+f"(d[3][5]), "+f"(d[3][6]), "+f"(d[3][7]), "+f"(d[3][8]), "+f"(d[3][9]), "+f"(d[3][10]), "+f"(d[3][11]), "+f"(d[3][12]), "+f"(d[3][13]), "+f"(d[3][14]), "+f"(d[3][15]), "+f"(d[3][16]), "+f"(d[3][17]), "+f"(d[3][18]), "+f"(d[3][19]), "+f"(d[3][20]), "+f"(d[3][21]), "+f"(d[3][22]), "+f"(d[3][23]), "+f"(d[3][24]), "+f"(d[3][25]), "+f"(d[3][26]), "+f"(d[3][27]), "+f"(d[3][28]), "+f"(d[3][29]), "+f"(d[3][30]), "+f"(d[3][31])
+#define BM_WGMMA(N, REGS) \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t" \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.bf16.bf16 {" REGS "}, %128, %129, p, %131, 1, %132, %133;\n\t}" \
+                 : BM_WG_ACC : "l"(da), "l"(db), "r"(scale_d), "n"(NEG ? -1 : 1), "n"(TA), "n"(TB))
+template <int BN16, int TA, int TB, int NEG>
+__device__ __forceinline__ void wgmma_k16(float (&d)[NB_MAX][32], uint64_t da, uint64_t db, uint32_t scale_d) {
+    static_assert(BN16 >= 1 && BN16 <= 16, "m64n16k16 .. m64n256k16");
+    if constexpr (BN16 == 1) BM_WGMMA(16, BM_WG_REGS_1);
+    else if constexpr (BN16 == 2) BM_WGMMA(32, BM_WG_REGS_2);
+    else if constexpr (BN16 == 3) BM_WGMMA(48, BM_WG_REGS_3);
+    else if constexpr (BN16 == 4) BM_WGMMA(64, BM_WG_REGS_4);
+    else if constexpr (BN16 == 5) BM_WGMMA(80, BM_WG_REGS_5);
+    else if constexpr (BN16 == 6) BM_WGMMA(96, BM_WG_REGS_6);
+    else if constexpr (BN16 == 7) BM_WGMMA(112, BM_WG_REGS_7);
+    else if constexpr (BN16 == 8) BM_WGMMA(128, BM_WG_REGS_8);
+    else if constexpr (BN16 == 9) BM_WGMMA(144, BM_WG_REGS_9);
+    else if constexpr (BN16 == 10) BM_WGMMA(160, BM_WG_REGS_10);
+    else if constexpr (BN16 == 11) BM_WGMMA(176, BM_WG_REGS_11);
+    else if constexpr (BN16 == 12) BM_WGMMA(192, BM_WG_REGS_12);
+    else if constexpr (BN16 == 13) BM_WGMMA(208, BM_WG_REGS_13);
+    else if constexpr (BN16 == 14) BM_WGMMA(224, BM_WG_REGS_14);
+    else if constexpr (BN16 == 15) BM_WGMMA(240, BM_WG_REGS_15);
+    else BM_WGMMA(256, BM_WG_REGS_16);
 }
 
 // Shared-memory matrix descriptor (wgmma): start address [0,14), leading byte offset [16,30), stride byte
@@ -278,26 +266,21 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, int mn_major)
     return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (lbo << 16) | (sbo << 32) | (1ull << 62);
 }
 
-// One K chunk (64) of the warpgroup's 64 x BN accumulator, BN = 16 BN16: 4 K=16 steps x (BN / 64 blocks of 64 columns + a
-// last block of BN % 64), as one wgmma group.  The A rows of warpgroup g and the B columns of block j both sit 8 KiB apart in
-// either layout (one 64-row / 64-column box each), and a K=16 step advances 32 B (K-major, inside the swizzle atom) or 2 KiB
-// (MN-major, two 8-k groups).  Every run-time choice is a template argument: a wgmma on a path ptxas cannot prove
-// warpgroup-uniform is serialised.
+// One K chunk (64) of the warpgroup's 64 x BN accumulator, BN = 16 BN16: 4 K=16 steps of one full-width wgmma each, as one wgmma
+// group, so each step reads the warpgroup's A fragment from shared memory once for the whole tile.  The A rows of warpgroup g
+// sit 8 KiB apart in either layout (one 64-row box each), an MN-major B tile is 64-column boxes 8 KiB apart (the descriptor's
+// leading byte offset), and a K=16 step advances 32 B (K-major, inside the swizzle atom) or 2 KiB (MN-major, two 8-k groups).
+// Every element's K order is that of four k16 steps, at any width.  Every run-time choice is a template argument: a wgmma on a
+// path ptxas cannot prove warpgroup-uniform is serialised.  Full-width instructions only: with one m64n64k16 per 64-column
+// block beside m64n256k16 on the same accumulators, ptxas 12.9 serialises every wgmma of the kernel (C7511).
 template <int TA, int TB, int NEG, int BN16>
 __device__ __forceinline__ void mma_chunk(float (&acc)[NB_MAX][32], uint32_t sA, uint32_t sB, uint32_t first) {
-    constexpr int NB = BN16 / 4, TAIL = 16 * (BN16 % 4);
     const uint32_t a_step = TA ? 2048u : 32u, b_step = TB ? 2048u : 32u;
     wg_fence();
 #pragma unroll
     for (int k = 0; k < BK / 16; ++k) {
-        const uint64_t da = make_smem_desc(sA + (uint32_t)k * a_step, TA);
         const uint32_t scale_d = (first && k == 0) ? 0u : 1u;
-#pragma unroll
-        for (int j = 0; j < NB; ++j)
-            wgmma_m64nk16<64, TA, TB, NEG>(acc[j], da, make_smem_desc(sB + (uint32_t)j * 8192u + (uint32_t)k * b_step, TB), scale_d);
-        if constexpr (TAIL > 0)
-            wgmma_m64nk16<(TAIL > 0 ? TAIL : 64), TA, TB, NEG>(acc[NB < NB_MAX ? NB : 0], da,
-                                                             make_smem_desc(sB + (uint32_t)NB * 8192u + (uint32_t)k * b_step, TB), scale_d);
+        wgmma_k16<BN16, TA, TB, NEG>(acc, make_smem_desc(sA + (uint32_t)k * a_step, TA), make_smem_desc(sB + (uint32_t)k * b_step, TB), scale_d);
     }
     wg_commit();
 }
@@ -1018,12 +1001,12 @@ static CUtensorMap make_map(const TcMat& m, int box0, int box1) {
 struct TilePick { int bn, cluster; };
 
 static TilePick pick_tile(int N, int m_tiles, int splits, int chunks, int sms, int force_cluster, int max_bn) {
-    // Tile width BN (64, 128 or 256: whole 64-column wgmma blocks and TMA-store granules) and row grouping (CTAs
-    // taking one 128-row block each, or pairs taking a 256-row group).  Cycle model per CTA:
+    // Tile width BN (64, 128 or 256: whole 64-column TMA-store granules) and row grouping (CTAs taking one 128-row block
+    // each, or pairs taking a 256-row group).  Cycle model per CTA:
     // waves * chunks * max(mma, ingest) + epilogue of the last tile, with the tensor cores at ~2048 bf16
     // MACs/clk per SM (989 TFLOP/s dense over 132 SMs) and operand ingest at ~32 B/clk per SM (measured on an H100 at
-    // 64, 128 and 256 columns alike, DESIGN 5.1): every width is ingest-bound, and a wider tile reads the A tile once
-    // for more columns -- 48 KiB per 1024 MMA cycles at BN = 256 against 32 KiB per 512 at BN = 128.
+    // 64 columns; with full-width wgmma 128- and 256-column tiles stream 41-47 B/clk, DESIGN 5.1): a wider tile reads the
+    // A tile once for more columns -- 48 KiB per 1024 MMA cycles at BN = 256 against 32 KiB per 512 at BN = 128.
     TilePick best{64, 1};
     double best_cost = 1e30;
     for (int c = 1; c <= 2; ++c) {
