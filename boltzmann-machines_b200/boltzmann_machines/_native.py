@@ -32,6 +32,7 @@ EXPORTS = (
     'bm_dbm_train_step', 'bm_dbm_val_metrics', 'bm_dbm_transform', 'bm_dbm_reconstruct', 'bm_dbm_log_proba',
     'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows', 'bm_dbm_ais_base', 'bm_dbm_ais_base_rows', 'bm_dbm_pt_counts', 'bm_debug_dbm_multinomial_rows',
     'bm_dbm_train_step_labeled', 'bm_dbm_predict_proba', 'bm_dbm_fill', 'bm_dbm_debug_last_fill', 'bm_dbm_debug_last_sample_v',
+    'bm_dbm_exact', 'bm_dbm_debug_exact_chunk',
     'bm_crbm_create', 'bm_crbm_destroy', 'bm_crbm_set_param', 'bm_crbm_get_param', 'bm_crbm_init_weights',
     'bm_crbm_train_step', 'bm_crbm_predict_proba', 'bm_crbm_transform', 'bm_crbm_debug_last_step',
     'bm_rbm_group_create', 'bm_rbm_group_destroy', 'bm_rbm_group_train_epoch', 'bm_rbm_group_train_epoch_u8',
@@ -173,6 +174,7 @@ def load_library(path=None):
         'bm_dbm_fill': [vp, vp, vp, vp, i32, u32, i32, u64, u32, vp],
         'bm_dbm_debug_last_fill': [vp, C.c_char_p, vp, sz],
         'bm_dbm_debug_last_sample_v': [vp, C.c_char_p, vp, sz],
+        'bm_dbm_exact': [vp, vp, i32, vp, vp], 'bm_dbm_debug_exact_chunk': [vp, i32],
         'bm_debug_dbm_multinomial_rows': [vp, vp, i32, i32, dbl, i32, u64, u32, u32, u32, vp, vp, vp, vp],
         'bm_crbm_create': [vp, C.POINTER(CrbmCfg), C.POINTER(vp)],
         'bm_crbm_set_param': [vp, C.c_char_p, vp, sz], 'bm_crbm_get_param': [vp, C.c_char_p, vp, sz],
@@ -1007,6 +1009,30 @@ class CudaDBM(object):
             check(self._lib.bm_dbm_ais_base_rows(self.handle, int(n_runs), int(n_betas), int(k), int(seed), int(first_run), bp,
                                                  out.ctypes.data))
         return out
+
+    def exact(self, X=None):
+        """Exact log p*(v) of X's rows (None: no rows) and log Z of a binary DBM with at most 32 odd-layer units, from one
+        enumeration of the odd layers' states (bm_dbm_exact, DESIGN.md §5.4f).  Returns (log_p_star [rows] float64 or None,
+        log_Z).  Refusals of the engine (BM_EUNSUPPORTED) raise NotImplementedError, bad arguments RuntimeError."""
+        lz = C.c_double(0.0)
+        if X is None:
+            rc = self._lib.bm_dbm_exact(self.handle, None, 0, None, C.byref(lz))
+            lp = None
+        else:
+            X = np.ascontiguousarray(X, dtype=np.float32)
+            if X.ndim != 2 or X.shape[1] != self.V:
+                raise ValueError('batch has shape {0}, expected (rows, {1})'.format(X.shape, self.V))
+            lp = np.empty(X.shape[0], dtype=np.float64)
+            rc = self._lib.bm_dbm_exact(self.handle, X.ctypes.data if len(X) else None, X.shape[0],
+                                        lp.ctypes.data if len(X) else None, C.byref(lz))
+        if rc == -5:                                  # BM_EUNSUPPORTED: the message names the reason
+            raise NotImplementedError('libbm: ' + self._lib.bm_last_error().decode('utf-8', 'replace'))
+        check(rc)
+        return lp, lz.value
+
+    def debug_exact_chunk(self, log2_states):
+        """states per launch of `exact`'s enumeration, 2^log2_states (0: the default) -- a test hook"""
+        check(self._lib.bm_dbm_debug_exact_chunk(self.handle, int(log2_states)))
 
     def close(self):
         if getattr(self, 'handle', None):

@@ -179,5 +179,11 @@ class ClassificationDBM(DBM):
     def log_Z(self, *args, **kwargs):
         raise NotImplementedError('ClassificationDBM: log_Z is not available (the AIS ladder has no label layer)')
 
+    def exact_log_Z(self, *args, **kwargs):
+        raise NotImplementedError('ClassificationDBM: exact_log_Z is not available (the enumeration has no label layer)')
+
+    def exact_log_proba(self, *args, **kwargs):
+        raise NotImplementedError('ClassificationDBM: exact_log_proba is not available (the enumeration has no label layer)')
+
     def log_proba(self, *args, **kwargs):
         raise NotImplementedError('ClassificationDBM: log_proba is not available (the variational bound has no label layer)')

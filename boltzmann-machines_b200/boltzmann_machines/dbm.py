@@ -467,6 +467,54 @@ class DBM(EnergyBasedModel):
         P = self._per_batch(X_test, 0, self._engine.log_proba, 'log_proba', np.float64)
         return P - log_Z
 
+    @run_in_tf_session()
+    def exact_log_Z(self):
+        """Exact log partition function of a binary DBM whose odd hidden layers h_1, h_3, ... hold at most 32 units together.
+
+        Every state of the odd layers is enumerated on the tensor-core engine, with v and the even layers summed out
+        analytically (DESIGN.md §5.4f), for the model as stored (float32 weights and biases).  A one-layer DBM is an RBM
+        with at most 32 hidden units.  Tempered and centered models need nothing extra.  Refusals raise
+        ``NotImplementedError`` naming the reason: non-binary layers, float64 models, ``compute='fp32'``, a
+        `ClassificationDBM`, or more than 32 odd-layer units."""
+        self._check_exact('exact_log_Z')
+        return float(self._engine.exact(None)[1])
+
+    @run_in_tf_session()
+    def exact_log_proba(self, X_test, log_Z=None):
+        """Exact log p(v) = log p*(v) - log Z of the rows of ``X_test`` [n, n_visible] (float64 [n]), for the models
+        `exact_log_Z` accepts.  The values of X are used as given, as in `log_proba`: for binary rows this is log p(v).
+        ``log_Z=None`` takes the exact log Z from the same enumeration.  Each slice of up to 16384 rows is one pass over
+        the states."""
+        self._check_exact('exact_log_proba')
+        X = np.asarray(X_test, dtype=np.float32)
+        if X.ndim != 2 or X.shape[1] != self.n_visible_:
+            raise ValueError('X_test has shape {0}, expected (n, {1})'.format(X.shape, self.n_visible_))
+        if not np.all(np.isfinite(X)):
+            raise ValueError('X_test must be finite')
+        out = np.empty(len(X), dtype=np.float64)
+        for lo in range(0, len(X), self._EXACT_ROWS):
+            hi = min(len(X), lo + self._EXACT_ROWS)
+            out[lo:hi], lz = self._engine.exact(X[lo:hi])
+            if log_Z is None:
+                log_Z = lz
+        if log_Z is None:                              # no rows
+            log_Z = self._engine.exact(None)[1]
+        return out - float(log_Z)
+
+    _EXACT_ROWS = 16384
+
+    def _check_exact(self, what):
+        """The refusals of bm_dbm_exact (include/bm.h), raised before the engine is called."""
+        if self.layers_['v']['kind'] != 'bernoulli' or any(h['kind'] != 'bernoulli' for h in self.layers_['h']):
+            raise NotImplementedError(what + ' is defined for binary layers (Bernoulli visible and hidden units)')
+        if np.dtype(self.dtype) != np.float32:
+            raise NotImplementedError(what + ' runs on the tensor-core engine: float32 models only')
+        if getattr(self._engine, 'compute', 'bf16') != 'bf16':
+            raise NotImplementedError(what + " runs on the tensor-core engine, not on the fp32 CUDA-core engine (compute='fp32')")
+        n_odd = sum(int(n) for n in self.n_hiddens_[0::2])
+        if n_odd > 32:
+            raise NotImplementedError('{0} enumerates the odd layers h_1, h_3, ...: n_odd = {1} units, at most 32'.format(what, n_odd))
+
     def _base_rates(self, base_rate):
         """log_Z's ``base_rate`` as one float32 vector or None per unit layer (v, h_1 .. h_L)"""
         widths = [self.n_visible_] + [int(n) for n in self.n_hiddens_]

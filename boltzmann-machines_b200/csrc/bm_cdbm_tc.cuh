@@ -155,6 +155,9 @@ struct ClassDbmTC : DbmTC {
         BM_CUDA(cudaMemcpyAsync(out, mu[Lm - 1].p, (size_t)rows * Hs[Lm - 1] * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
         BM_CUDA(cudaStreamSynchronize(ctx->stream));
     }
+    void exact(const void*, int, double*, double*) override {
+        throw Error(BM_EUNSUPPORTED, "classification DBM: exact log Z is not supported (the enumeration has no label layer)");
+    }
     void log_proba(const void*, int, double*) override {
         throw Error(BM_EUNSUPPORTED, "classification DBM: log_proba is not supported (the variational bound has no label layer)");
     }

@@ -266,6 +266,11 @@ struct DbmBase {
                       uint32_t tick, void* out) = 0;
     virtual void fill_debug(const char* name, void* host, size_t bytes) = 0;
     virtual void sample_v_debug(const char* name, void* host, size_t bytes) = 0;
+    // exact log Z and log p*(v) by enumerating the odd layers (DESIGN.md §5.4f): the tensor-core engine's (bm_dbm_exact.cuh)
+    virtual void exact(const void*, int, double*, double*) {
+        throw Error(BM_EUNSUPPORTED, "exact log Z runs on the tensor-core engine (float32 models, BM_COMPUTE_BF16), not on the "
+                                     "CUDA-core engine");
+    }
 };
 
 // Parallel tempering (bm_dbm_cfg.n_temps / betas): what the engines refuse before anything is allocated.  0 / NULL is off.
@@ -876,6 +881,7 @@ struct Dbm : DbmBase {
 #include "bm_dbm_tc.cuh"     // DbmTC: the same engine with every GEMM on the tensor cores (opt-in)
 #include "bm_crbm_tc.cuh"    // ClassRbmTC: the classification RBM, a DbmTC of shape x - h - label (bm_crbm_*)
 #include "bm_cdbm_tc.cuh"    // ClassDbmTC: the classification DBM, a DbmTC with a label layer on top (bm_dbm_cfg.n_classes)
+#include "bm_dbm_exact.cuh"   // DbmTC::exact: exact log Z and log p*(v) over the odd layers' states (bm_dbm_exact)
 
 using namespace bm;
 
@@ -989,6 +995,17 @@ int bm_dbm_fill(bm_dbm* h, const void* X, const uint8_t* mask, const int32_t* la
 }
 int bm_dbm_debug_last_fill(bm_dbm* h, const char* name, void* host, size_t bytes) {
     BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(name && host, "null argument"); DBM(h)->fill_debug(name, host, bytes); BM_API_END
+}
+int bm_dbm_exact(bm_dbm* h, const void* X, int32_t rows, double* log_p_star, double* log_Z) {
+    BM_API_BEGIN DBM_ENTER(h) DBM(h)->exact(X, rows, log_p_star, log_Z); BM_API_END
+}
+int bm_dbm_debug_exact_chunk(bm_dbm* h, int32_t log2_states) {
+    BM_API_BEGIN DBM_ENTER(h)
+    DbmTC* d = dynamic_cast<DbmTC*>(DBM(h));
+    if (!d) throw Error(BM_EUNSUPPORTED, "exact log Z runs on the tensor-core engine");
+    BM_REQUIRE(log2_states == 0 || (log2_states >= 1 && log2_states <= 30), "exact chunk: log2 of the states per launch in [1, 30], or 0");
+    d->exact_chunk_bits = log2_states == 0 ? DbmTC::EXACT_CHUNK_BITS : log2_states;
+    BM_API_END
 }
 int bm_dbm_debug_last_sample_v(bm_dbm* h, const char* name, void* host, size_t bytes) {
     BM_API_BEGIN DBM_ENTER(h) BM_REQUIRE(name && host, "null argument"); DBM(h)->sample_v_debug(name, host, bytes); BM_API_END

@@ -539,6 +539,11 @@ struct DbmTC : Dbm<float> {
         return f.n_layers <= TC_PROGRAM_OPS;     // one mean-field sweep (L ops) fits in one program
     }
     bool multinomial(int i) const { return h_kinds[i] == BM_UNIT_MULTINOMIAL; }
+    // exact log Z / log p*(v) (bm_dbm_exact.cuh): 2^exact_chunk_bits states per launch of the enumeration (bounds g and the
+    // rows' pairs); bm_dbm_debug_exact_chunk lowers it so that small models span several launches
+    static constexpr int EXACT_CHUNK_BITS = 22;
+    int exact_chunk_bits = EXACT_CHUNK_BITS;
+    void exact(const void* X, int rows, double* log_p_star, double* log_Z) override;
 
     DbmTC(Ctx* c, const bm_dbm_cfg& f) : Dbm<float>(c, f) {
         if (f.n_temps >= 1) {                    // validated by bm_dbm_create (check_pt_cfg)

@@ -295,6 +295,19 @@ int  bm_dbm_ais_base(bm_dbm* dbm, int32_t n_runs, int32_t n_betas, int32_t n_gib
                      double* logZ);
 int  bm_dbm_ais_base_rows(bm_dbm* dbm, int32_t n_runs, int32_t n_betas, int32_t n_gibbs_steps, uint64_t seed, uint32_t first_run,
                           const float* const* base, double* logZ);
+/* Exact log Z and log p*(v) of a binary DBM whose odd layers h_1, h_3, ... hold n_odd <= 32 units (DESIGN.md §5.4f): every
+ * state x of the odd layers is enumerated on the tensor cores, v and the even layers summed out analytically, for the model
+ * as stored (float32 W and biases, not the bf16 shadow the chains read).  X [rows, n_visible] float32 (used as given, so grey
+ * rows are allowed); log_p_star [rows] receives log p*(v) = log sum_h exp(-E(v, h)) (without -log Z) and log_Z, if not NULL,
+ * log Z -- both from one pass over the states.  X = NULL, rows = 0 computes log Z only.  Every rank of a context with a
+ * communicator computes the whole sum and gets the same result.  Refused before any launch: BM_EINVAL for rows < 0, a missing
+ * X or log_p_star with rows > 0, X with rows = 0, nothing to compute, or a non-finite entry of X; BM_EUNSUPPORTED (the reason
+ * named) for the CUDA-core engine (float64 models, BM_COMPUTE_FP32), Gaussian visibles or multinomial layers, classification
+ * DBMs and n_odd > 32. */
+int  bm_dbm_exact(bm_dbm* dbm, const void* X, int32_t rows, double* log_p_star, double* log_Z);
+/* test hook: 2^log2_states states per launch of bm_dbm_exact's enumeration (1..30; 0 restores the default 2^22), so that
+ * small models span several launches.  The result does not depend on it beyond float64 rounding. */
+int  bm_dbm_debug_exact_chunk(bm_dbm* dbm, int32_t log2_states);
 /* parallel tempering: swaps accepted / proposed between slots m and m+1 since create, n_temps-1 entries each (BM_EINVAL
  * without tempering) */
 int  bm_dbm_pt_counts(bm_dbm* dbm, int64_t* accepted, int64_t* proposed);
