@@ -32,7 +32,7 @@ EXPORTS = (
     'bm_dbm_train_step', 'bm_dbm_val_metrics', 'bm_dbm_transform', 'bm_dbm_reconstruct', 'bm_dbm_log_proba',
     'bm_dbm_sample_v', 'bm_dbm_ais', 'bm_dbm_ais_rows', 'bm_dbm_ais_base', 'bm_dbm_ais_base_rows', 'bm_dbm_pt_counts', 'bm_debug_dbm_multinomial_rows',
     'bm_dbm_train_step_labeled', 'bm_dbm_predict_proba', 'bm_dbm_fill', 'bm_dbm_debug_last_fill', 'bm_dbm_debug_last_sample_v',
-    'bm_dbm_exact', 'bm_dbm_debug_exact_chunk',
+    'bm_dbm_exact', 'bm_dbm_debug_exact_chunk', 'bm_dbm_ais_clamped',
     'bm_crbm_create', 'bm_crbm_destroy', 'bm_crbm_set_param', 'bm_crbm_get_param', 'bm_crbm_init_weights',
     'bm_crbm_train_step', 'bm_crbm_predict_proba', 'bm_crbm_transform', 'bm_crbm_debug_last_step',
     'bm_rbm_group_create', 'bm_rbm_group_destroy', 'bm_rbm_group_train_epoch', 'bm_rbm_group_train_epoch_u8',
@@ -175,6 +175,7 @@ def load_library(path=None):
         'bm_dbm_debug_last_fill': [vp, C.c_char_p, vp, sz],
         'bm_dbm_debug_last_sample_v': [vp, C.c_char_p, vp, sz],
         'bm_dbm_exact': [vp, vp, i32, vp, vp], 'bm_dbm_debug_exact_chunk': [vp, i32],
+        'bm_dbm_ais_clamped': [vp, vp, i32, u32, i32, i32, i32, u64, vp],
         'bm_debug_dbm_multinomial_rows': [vp, vp, i32, i32, dbl, i32, u64, u32, u32, u32, vp, vp, vp, vp],
         'bm_crbm_create': [vp, C.POINTER(CrbmCfg), C.POINTER(vp)],
         'bm_crbm_set_param': [vp, C.c_char_p, vp, sz], 'bm_crbm_get_param': [vp, C.c_char_p, vp, sz],
@@ -1029,6 +1030,21 @@ class CudaDBM(object):
             raise NotImplementedError('libbm: ' + self._lib.bm_last_error().decode('utf-8', 'replace'))
         check(rc)
         return lp, lz.value
+
+    def ais_clamped(self, X, n_runs, n_betas, k, seed, row0=0):
+        """Per-run AIS estimates of log p*(v) for the rows of X with v clamped (bm_dbm_ais_clamped, DESIGN.md §5.4g):
+        [rows, n_runs] float64, log Z_0 and b_v.v included; the rows are rows row0.. of the caller's data.  Refusals of the
+        engine (BM_EUNSUPPORTED) raise NotImplementedError, bad arguments RuntimeError."""
+        X = np.ascontiguousarray(X, dtype=np.float32)
+        if X.ndim != 2 or X.shape[1] != self.V:
+            raise ValueError('batch has shape {0}, expected (rows, {1})'.format(X.shape, self.V))
+        out = np.empty((X.shape[0], max(int(n_runs), 0)), dtype=np.float64)
+        rc = self._lib.bm_dbm_ais_clamped(self.handle, X.ctypes.data if X.size else None, X.shape[0], int(row0), int(n_runs),
+                                          int(n_betas), int(k), int(seed), out.ctypes.data if out.size else None)
+        if rc == -5:                                  # BM_EUNSUPPORTED: the message names the reason
+            raise NotImplementedError('libbm: ' + self._lib.bm_last_error().decode('utf-8', 'replace'))
+        check(rc)
+        return out
 
     def debug_exact_chunk(self, log2_states):
         """states per launch of `exact`'s enumeration, 2^log2_states (0: the default) -- a test hook"""

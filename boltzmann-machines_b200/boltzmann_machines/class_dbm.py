@@ -187,3 +187,6 @@ class ClassificationDBM(DBM):
 
     def log_proba(self, *args, **kwargs):
         raise NotImplementedError('ClassificationDBM: log_proba is not available (the variational bound has no label layer)')
+
+    def ais_log_proba(self, *args, **kwargs):
+        raise NotImplementedError('ClassificationDBM: ais_log_proba is not available (the AIS ladder has no label layer)')

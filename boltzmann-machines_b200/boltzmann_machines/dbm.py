@@ -503,6 +503,52 @@ class DBM(EnergyBasedModel):
 
     _EXACT_ROWS = 16384
 
+    @run_in_tf_session(update_seed=True)
+    def ais_log_proba(self, X_test, log_Z, n_betas=100, n_runs=100, n_gibbs_steps=5, return_runs=False):
+        """AIS estimate of log p(v) for the rows of ``X_test`` [n, n_visible] given an estimate of log Z (DESIGN.md §5.4g;
+        Salakhutdinov & Hinton 2009).
+
+        Each row runs ``n_runs`` AIS chains with v clamped to it: the odd hidden layers h_1, h_3, ... are summed out
+        analytically and the even ones are annealed from the uniform model to the DBM, with the temperatures and sweeps of
+        `log_Z` (whose defaults these are, so the two read alike; trained models want far more temperatures than 100).  Like
+        `log_Z`'s ladder it weighs each state at the temperature it was just drawn at, which biases the estimate up by
+        O(1 / n_betas): +0.08 nats at 1000 temperatures on a trained 784-24-1000 model, +0.8 at 100.  `log_proba`'s bound
+        sits below log p(v) by the variational gap instead.  Every layer the chains draw is sampled, whatever
+        ``sample_h_states`` says.  The values of X are used as given, as in `log_proba`; grey rows enter the products as bf16.
+        A one-layer DBM has nothing to anneal: every run is `log_proba`'s value, which is exact there.
+
+        Runs on the tensor-core engine (float32 models, ``compute='bf16'``) with binary layers; otherwise
+        ``NotImplementedError`` names what is missing.  Tempered and centered models need nothing extra.  A row's runs
+        depend only on its index in ``X_test`` and the call's seed.  Returns float64 [n]: each row's log-mean-exp over its
+        runs minus ``log_Z``; with ``return_runs=True`` also the [n, n_runs] per-run estimates of log p*(v).
+        """
+        self._check_depth('ais_log_proba', ais=False, clamped=True)
+        X = np.asarray(X_test, dtype=np.float32)
+        if X.ndim != 2 or X.shape[1] != self.n_visible_:
+            raise ValueError('X_test has shape {0}, expected (n, {1})'.format(X.shape, self.n_visible_))
+        if not np.all(np.isfinite(X)):
+            raise ValueError('X_test must be finite')
+        n_runs, n_betas, k = int(n_runs), int(n_betas), int(n_gibbs_steps)
+        if n_runs < 1 or n_betas < 2 or k < 1:
+            raise ValueError('ais_log_proba needs n_runs >= 1, n_betas >= 2 and n_gibbs_steps >= 1')
+        seed = self.make_random_seed()
+        runs = np.empty((len(X), n_runs), dtype=np.float64)
+        step = max(1, self._AIS_CLAMPED_CHAINS // n_runs)
+        keep = self._snapshot() if self.n_layers_ == 1 else None      # one layer: the engine's log_proba writes the E-step's means
+        try:
+            for lo in range(0, len(X), step):
+                hi = min(len(X), lo + step)
+                runs[lo:hi] = self._engine.ais_clamped(X[lo:hi], n_runs, n_betas, k, seed, row0=lo)
+        finally:
+            if keep is not None:
+                self._engine.set_params(keep)
+        m = runs.max(axis=1, keepdims=True)
+        est = (m[:, 0] + np.log(np.mean(np.exp(runs - m), axis=1))) - float(log_Z)
+        return (est, runs) if return_runs else est
+
+    # chains per engine call of ais_log_proba (DbmTC::AIS_CLAMPED_CHAINS: one ladder slice; at least log_Z's 20 000 runs)
+    _AIS_CLAMPED_CHAINS = 32768
+
     def _check_exact(self, what):
         """The refusals of bm_dbm_exact (include/bm.h), raised before the engine is called."""
         if self.layers_['v']['kind'] != 'bernoulli' or any(h['kind'] != 'bernoulli' for h in self.layers_['h']):
@@ -541,10 +587,10 @@ class DBM(EnergyBasedModel):
         p = (X.sum(axis=0) + 1.) / (X.shape[0] + 2.)
         return [np.log(p / (1. - p)).astype(np.float32)] + [None] * self.n_layers_
 
-    def _check_depth(self, what, ais):
+    def _check_depth(self, what, ais, clamped=False):
         """The refusals of the engine (include/bm.h, bm_dbm_ais / bm_dbm_ais_base / bm_dbm_log_proba) at a depth other than 2,
-        and of AIS from a base-rate model at any depth."""
-        where = what if 'base-rate' in what else '{0} at {1} hidden layers'.format(what, self.n_layers_)
+        of AIS from a base-rate model at any depth and, with ``clamped``, of bm_dbm_ais_clamped at any depth."""
+        where = what if ('base-rate' in what or clamped) else '{0} at {1} hidden layers'.format(what, self.n_layers_)
         if self.layers_['v']['kind'] != 'bernoulli' or any(h['kind'] != 'bernoulli' for h in self.layers_['h']):
             raise NotImplementedError(where + ' is defined for binary layers (Bernoulli visible and hidden units)')
         if np.dtype(self.dtype) != np.float32:

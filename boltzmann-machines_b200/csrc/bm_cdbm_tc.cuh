@@ -161,6 +161,9 @@ struct ClassDbmTC : DbmTC {
     void log_proba(const void*, int, double*) override {
         throw Error(BM_EUNSUPPORTED, "classification DBM: log_proba is not supported (the variational bound has no label layer)");
     }
+    void ais_clamped(const void*, int, uint32_t, int, int, int, uint64_t, double*) override {
+        throw Error(BM_EUNSUPPORTED, "classification DBM: AIS with v clamped is not supported (the AIS ladder has no label layer)");
+    }
     void ais(int, int, int, uint64_t, const float* const*, double*) override {
         throw Error(BM_EUNSUPPORTED, "classification DBM: AIS is not supported (the AIS ladder has no label layer)");
     }

@@ -271,6 +271,11 @@ struct DbmBase {
         throw Error(BM_EUNSUPPORTED, "exact log Z runs on the tensor-core engine (float32 models, BM_COMPUTE_BF16), not on the "
                                      "CUDA-core engine");
     }
+    // AIS over the hidden layers with v clamped to each row of X (DESIGN.md §5.4g): the tensor-core engine's (DbmTC)
+    virtual void ais_clamped(const void*, int, uint32_t, int, int, int, uint64_t, double*) {
+        throw Error(BM_EUNSUPPORTED, "AIS with v clamped runs on the tensor-core engine (float32 models, BM_COMPUTE_BF16), not on "
+                                     "the CUDA-core engine");
+    }
 };
 
 // Parallel tempering (bm_dbm_cfg.n_temps / betas): what the engines refuse before anything is allocated.  0 / NULL is off.
@@ -998,6 +1003,10 @@ int bm_dbm_debug_last_fill(bm_dbm* h, const char* name, void* host, size_t bytes
 }
 int bm_dbm_exact(bm_dbm* h, const void* X, int32_t rows, double* log_p_star, double* log_Z) {
     BM_API_BEGIN DBM_ENTER(h) DBM(h)->exact(X, rows, log_p_star, log_Z); BM_API_END
+}
+int bm_dbm_ais_clamped(bm_dbm* h, const void* X, int32_t rows, uint32_t row0, int32_t n_runs, int32_t n_betas,
+                       int32_t n_gibbs_steps, uint64_t seed, double* log_w) {
+    BM_API_BEGIN DBM_ENTER(h) DBM(h)->ais_clamped(X, rows, row0, n_runs, n_betas, n_gibbs_steps, seed, log_w); BM_API_END
 }
 int bm_dbm_debug_exact_chunk(bm_dbm* h, int32_t log2_states) {
     BM_API_BEGIN DBM_ENTER(h)

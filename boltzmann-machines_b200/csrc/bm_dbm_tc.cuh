@@ -303,6 +303,17 @@ __global__ void ais_unit_bf16_kernel(const float* __restrict__ pre, int ldp, flo
     *reinterpret_cast<uint2*>(out + (size_t)r * ldo + cb * 4) = pk;       // columns >= cols land in the padding
 }
 
+// v's operand of the clamped AIS ladder (DESIGN.md §5.4g): chain i of a slice is chain c0 + i of the call, which reads row
+// (c0 + i) / n_runs of X [rows, V] (float32, device).  out [n, ldo] bf16 with the padding columns zero; binary rows are exact.
+__global__ void ais_clamp_rows_kernel(const float* __restrict__ X, int V, long long c0, int n_runs, bf16_t* __restrict__ out,
+                                      int ldo, int n) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    const int i = blockIdx.y;
+    if (c >= ldo || i >= n) return;
+    const float* x = X + (size_t)((c0 + i) / n_runs) * V;
+    out[(size_t)i * ldo + c] = __float2bfloat16_rn(c < V ? x[c] : 0.f);
+}
+
 // softplus(b z) - softplus(a z), b >= a >= 0, without cancellation
 __device__ __forceinline__ float softplus_diff(float a, float b, float z) {
     const float s = 1.0f / (1.0f + expf(-a * z));          // sigmoid(a z)
@@ -1572,10 +1583,17 @@ struct DbmTC : Dbm<float> {
     // With a base-rate model (DESIGN.md §5.4d; base: NULL or L + 1 nullable host vectors a_j) the path runs from
     // p_A ∝ exp(sum_j a_j.x_j): every op reads u_j = z_j - a_j, i.e. the bias b_j - a_j, and adds a_j after the beta scaling in
     // its epilogue (TcGemm::ais_base); the initial states are drawn from sigmoid(a_j).
-    void ais_local_layers(int R, uint32_t row0, int n_betas, int k, uint64_t seed, const float* const* base, double* logw_out) {
+    // With v clamped (DESIGN.md §5.4g; clamp: the bf16 rows of v [R, ldn[0]], no base) the roles move up one layer: v is a
+    // constant operand, the odd layers are summed out and the even layers h_2, h_4, ... are the state.  Every layer drawn is
+    // sampled, whatever sample_h says, and every draw is at SITE_AIS_CLAMPED: t = 2 j for the initial state of layer j, 2 j + 1
+    // for its transition draws.
+    void ais_local_layers(int R, uint32_t row0, int n_betas, int k, uint64_t seed, const float* const* base, double* logw_out,
+                          const bf16_t* clamp = nullptr) {
         const int NL = L + 1;
         auto width = [&](int j) { return j == 0 ? V : Hs[j - 1]; };
         auto slot = [&](int j) { return (uint32_t)((j - 1) / 2); };
+        std::vector<int> summed, state;                                   // the layers' roles, each in increasing j
+        for (int j = clamp ? 1 : 0; j < NL; ++j) ((j % 2 == 1) == (clamp != nullptr) ? summed : state).push_back(j);
         std::vector<const float*> bias(NL), abase(NL, nullptr);
         std::vector<DevBuf<float>> a_dev(NL), d_dev(NL);
         std::vector<std::vector<float>> d_host(NL);
@@ -1594,15 +1612,17 @@ struct DbmTC : Dbm<float> {
         }
         std::vector<DevBuf<bf16_t>> buf(NL), buf2(NL);
         std::vector<bf16_t*> cur(NL), nxt(NL);
-        for (int j = 0; j < NL; ++j) {
+        if (clamp) cur[0] = nxt[0] = const_cast<bf16_t*>(clamp);                // read only
+        for (int j = clamp ? 1 : 0; j < NL; ++j) {
             buf[j].ensure((size_t)R * ldn[j]); buf[j].zero(ctx->stream);
             cur[j] = nxt[j] = buf[j].p;
-            if (j % 2) { buf2[j].ensure((size_t)R * ldn[j]); buf2[j].zero(ctx->stream); nxt[j] = buf2[j].p; }
         }
-        for (int j = 1; j < NL; j += 2) {       // x_0 ~ Ber(1/2)   (:700-702), or Ber(sigmoid(a_j)): a_j broadcast to every run
+        for (int j : state) { buf2[j].ensure((size_t)R * ldn[j]); buf2[j].zero(ctx->stream); nxt[j] = buf2[j].p; }
+        for (int j : state) {                   // x_0 ~ Ber(1/2)   (:700-702), or Ber(sigmoid(a_j)): a_j broadcast to every run
             dim3 g(((width(j) + 3) / 4 + 127) / 128, R);
             ais_unit_bf16_kernel<<<g, 128, 0, ctx->stream>>>(abase[j], 0, abase[j] ? 1.f : 0.f, cur[j], ldn[j], R, width(j), 1,
-                                                             make_rng(seed, SITE_AIS_INIT, slot(j), 0, row0));
+                                                             clamp ? make_rng(seed, SITE_AIS_CLAMPED, 2 * j, 0, row0)
+                                                                   : make_rng(seed, SITE_AIS_INIT, slot(j), 0, row0));
             count_launch(ctx);
         }
         // the temperatures, as ais_local accumulates them
@@ -1639,10 +1659,11 @@ struct DbmTC : Dbm<float> {
             g.ais_kind = 1; g.ais_a = a; g.ais_b = b; g.ais_next = next; g.ais_logw = weigh ? logw_out : nullptr;
             g.tick_off = tick;
             if (emit) {
-                const bool smp = j == 0 ? sample_vis != 0 : sample_h[j - 1] != 0;
+                const bool smp = clamp || (j == 0 ? sample_vis != 0 : sample_h[j - 1] != 0);
                 g.sample = smp ? SMP_BERNOULLI : SMP_NONE;
                 g.out_state_bf = cur[j]; g.ld_state_bf = ldn[j];
-                g.rng = j == 0 ? make_rng(0, SITE_AIS_V, 0, 0, 0) : make_rng(0, SITE_AIS_H2, slot(j), 0, 0);
+                g.rng = clamp ? make_rng(0, SITE_AIS_CLAMPED, 2 * j + 1, 0, 0)
+                              : j == 0 ? make_rng(0, SITE_AIS_V, 0, 0, 0) : make_rng(0, SITE_AIS_H2, slot(j), 0, 0);
                 last[j] = (int)all.size();
             }
             all.push_back(g);
@@ -1652,12 +1673,12 @@ struct DbmTC : Dbm<float> {
                 const uint32_t tick = (uint32_t)(s * k + sw);
                 const bool weigh = sw == 0 && s >= 1;                    // the increment of x_s (produced by transition s-1)
                 const float a = weigh ? inc_a(s - 1) : 0.f, b = weigh ? inc_b(s - 1) : 0.f;
-                for (int j = 0; j < NL; j += 2) unit_op(j, a, b, weigh, t[s], true, tick);
-                for (int j = 1; j < NL; j += 2) {                         // x'_j ~ sigmoid(beta (z_j - c_j) + beta c_j)
+                for (int j : summed) unit_op(j, a, b, weigh, t[s], true, tick);
+                for (int j : state) {                                     // x'_j ~ sigmoid(beta (z_j - c_j) + beta c_j)
                     TcGemm o = layer_op(j, cur);
                     o.acc_scale = t[s]; o.bias_scale = t[s]; o.act = ACT_SIGMOID;
                     o.sample = SMP_BERNOULLI; o.out_state_bf = nxt[j]; o.ld_state_bf = ldn[j];
-                    o.rng = make_rng(0, SITE_AIS_H1, slot(j), 0, 0);
+                    o.rng = clamp ? make_rng(0, SITE_AIS_CLAMPED, 2 * j + 1, 0, 0) : make_rng(0, SITE_AIS_H1, slot(j), 0, 0);
                     o.tick_off = tick;
                     o.ais_kind = 2;
                     if (sw == k - 1) {
@@ -1670,7 +1691,7 @@ struct DbmTC : Dbm<float> {
                 }
             }
         }
-        for (int j = 0; j < NL; j += 2) unit_op(j, inc_a(nT - 1), inc_b(nT - 1), true, 0.f, false, 0);    // :728
+        for (int j : summed) unit_op(j, inc_a(nT - 1), inc_b(nT - 1), true, 0.f, false, 0);               // :728
         // launches of up to TC_PROGRAM_OPS ops; a dependency on an op of an earlier launch is the kernel boundary
         TcProgram prog;
         for (size_t lo = 0; lo < all.size(); lo += (size_t)TC_PROGRAM_OPS) {
@@ -1686,6 +1707,64 @@ struct DbmTC : Dbm<float> {
             launch_tc_program(ctx, prog, make_rng(seed, 0, 0, 0, row0), 0);
         }
         BM_CUDA(cudaStreamSynchronize(ctx->stream));            // the workspaces above are released on return
+    }
+
+    // ---- AIS with v clamped (DESIGN.md §5.4g) -------------------------------------------------------------------------
+    // Chain c = r n_runs + k is run k of row r; it draws from Philox row (row0 + r) n_runs + k, so a row's runs depend only on
+    // its index in the caller's data.  The chains run in slices of at most AIS_CLAMPED_CHAINS consecutive chains: one ladder
+    // of ais_local_layers each, on v's bf16 operand built for the slice.  log_w[c] = log Z_0 + b_v.X_r + the increments, with
+    // log Z_0 = (sum_i H_i) log 2 and b_v.X_r in float64 on the host from the float32 X.  At L = 1 there is nothing to
+    // anneal: every run is log_proba's value, exact there (and, as log_proba does, the call writes the E-step's means).
+    static constexpr int AIS_CLAMPED_CHAINS = 32768;
+    void ais_clamped(const void* Xh, int rows, uint32_t row0, int n_runs, int n_betas, int k, uint64_t seed, double* log_w) override {
+        bool binary = v_kind == BM_UNIT_BERNOULLI;
+        for (int i = 0; i < L; ++i) binary = binary && h_kinds[i] == BM_UNIT_BERNOULLI;
+        if (!binary) throw Error(BM_EUNSUPPORTED, "AIS with v clamped is defined for binary layers (Bernoulli visible and hidden units)");
+        BM_REQUIRE(rows >= 1 && n_runs >= 1 && n_betas >= 2 && k >= 1, "bad AIS arguments");
+        BM_REQUIRE(Xh && log_w, "ais_clamped: null argument");
+        BM_REQUIRE(((uint64_t)row0 + (uint64_t)rows) * (uint64_t)n_runs < (1ull << 32),
+                   "ais_clamped: (row0 + rows) * n_runs must stay below 2^32 (the chains' Philox rows)");
+        const float* X = static_cast<const float*>(Xh);
+        for (size_t i = 0; i < (size_t)rows * V; ++i)
+            BM_REQUIRE(std::isfinite(X[i]), "ais_clamped: X has a non-finite entry");
+        const long long total = (long long)rows * n_runs;
+        if (L == 1) {
+            std::vector<double> lp(B);
+            for (int lo = 0; lo < rows; lo += B) {
+                const int n = std::min(B, rows - lo);
+                log_proba(X + (size_t)lo * V, n, lp.data());
+                for (int r = 0; r < n; ++r) std::fill(log_w + (size_t)(lo + r) * n_runs, log_w + (size_t)(lo + r + 1) * n_runs, lp[r]);
+            }
+            return;
+        }
+        std::vector<float> b_v(V);
+        BM_CUDA(cudaMemcpyAsync(b_v.data(), vb.p, (size_t)V * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+        DevBuf<float> Xd;
+        Xd.ensure((size_t)rows * V);
+        BM_CUDA(cudaMemcpyAsync(Xd.p, X, (size_t)rows * V * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+        BM_CUDA(cudaStreamSynchronize(ctx->stream));
+        const int cap = (int)std::min<long long>(total, AIS_CLAMPED_CHAINS);
+        DevBuf<bf16_t> vop;
+        DevBuf<double> lw;
+        vop.ensure((size_t)cap * ldn[0]); lw.ensure(cap);
+        std::vector<double> hw(cap);
+        double logZ0 = 0.0;
+        for (int i = 0; i < L; ++i) logZ0 += (double)Hs[i] * 0.69314718055994530942;
+        for (long long c0 = 0; c0 < total; c0 += cap) {
+            const int n = (int)std::min<long long>(cap, total - c0);
+            ais_clamp_rows_kernel<<<dim3((ldn[0] + 127) / 128, n), 128, 0, ctx->stream>>>(Xd.p, V, c0, n_runs, vop.p, ldn[0], n);
+            count_launch(ctx);
+            lw.zero(ctx->stream);
+            ais_local_layers(n, (uint32_t)((uint64_t)row0 * n_runs + (uint64_t)c0), n_betas, k, seed, nullptr, lw.p, vop.p);
+            BM_CUDA(cudaMemcpyAsync(hw.data(), lw.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+            BM_CUDA(cudaStreamSynchronize(ctx->stream));
+            for (int i = 0; i < n; ++i) {
+                const long long r = (c0 + i) / n_runs;
+                double bvx = 0.0;
+                for (int c = 0; c < V; ++c) bvx += (double)b_v[c] * (double)X[(size_t)r * V + c];
+                log_w[c0 + i] = hw[i] + logZ0 + bvx;
+            }
+        }
     }
 
     // the same ladder for models whose first hidden layer is not sampled: fp32 pre-activations in memory and, per temperature,

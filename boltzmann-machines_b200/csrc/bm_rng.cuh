@@ -21,6 +21,7 @@ enum Site : uint32_t {
     SITE_MULTINOMIAL_FE = 5, SITE_PARTICLE_INIT = 6, SITE_AIS_INIT = 7,
     SITE_AIS_V = 8, SITE_AIS_H2 = 9, SITE_AIS_H1 = 10, SITE_DBM_V = 11, SITE_CRBM_Y = 12, SITE_CRBM_Y0 = 13,
     SITE_DBM_PT = 14,        // parallel tempering: the swap decision of pair (m, m+1) at t = m, column 0 of the particle's row
+    SITE_AIS_CLAMPED = 15,   // AIS with v clamped: layer j's initial state at t = 2 j, its transition draws at t = 2 j + 1
     SITE_DBM_H = 16
 };
 

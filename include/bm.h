@@ -305,6 +305,22 @@ int  bm_dbm_ais_base_rows(bm_dbm* dbm, int32_t n_runs, int32_t n_betas, int32_t 
  * named) for the CUDA-core engine (float64 models, BM_COMPUTE_FP32), Gaussian visibles or multinomial layers, classification
  * DBMs and n_odd > 32. */
 int  bm_dbm_exact(bm_dbm* dbm, const void* X, int32_t rows, double* log_p_star, double* log_Z);
+/* DESIGN.md §5.4g: AIS over the hidden layers with v clamped to each row of X [rows, n_visible] float32.
+ * log_w [rows * n_runs] receives each run's estimate of log p*(v_r) (log Z_0 and b_v.v included).
+ * An estimate of the true log p*(v) = log sum_h exp(-E(v, h)) of a binary DBM of any depth, where log_proba gives a lower
+ * bound: Salakhutdinov & Hinton (2009) run this ladder on each test vector; the reference has nothing like it.  With v fixed
+ * the odd layers h_1, h_3, ... are summed out analytically and the even layers h_2, h_4, ... are the chains' state; every
+ * layer drawn is sampled, whatever sample_h says.  Temperatures, sweeps and increments are those of bm_dbm_ais, on the bf16
+ * shadow of W; log Z_0 = (sum_i H_i) log 2 and b_v.v are added in float64.  X is used as given: grey rows enter the X W_0
+ * product as bf16(X).  Entry c = r * n_runs + k is run k of row r; it draws from Philox row (row0 + r) * n_runs + k, so a
+ * row's runs depend only on its global index row0 + r, never on how the caller slices the rows.  At one hidden layer there
+ * is nothing to anneal: every run is bm_dbm_log_proba's value, exact there, and the call writes the E-step's means as that
+ * call does; otherwise it reads W and the biases only.  No communication: each rank computes the call it was given.
+ * Refused before any launch: BM_EUNSUPPORTED (the reason named) on the CUDA-core engine (float64 models, BM_COMPUTE_FP32),
+ * for Gaussian visibles or multinomial layers and for classification DBMs; BM_EINVAL for a NULL X or log_w, rows < 1,
+ * n_runs < 1, n_betas < 2, n_gibbs_steps < 1, a non-finite entry of X, or (row0 + rows) * n_runs >= 2^32. */
+int  bm_dbm_ais_clamped(bm_dbm* dbm, const void* X, int32_t rows, uint32_t row0, int32_t n_runs, int32_t n_betas,
+                        int32_t n_gibbs_steps, uint64_t seed, double* log_w);
 /* test hook: 2^log2_states states per launch of bm_dbm_exact's enumeration (1..30; 0 restores the default 2^22), so that
  * small models span several launches.  The result does not depend on it beyond float64 rounding. */
 int  bm_dbm_debug_exact_chunk(bm_dbm* dbm, int32_t log2_states);

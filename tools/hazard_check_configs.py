@@ -1,6 +1,6 @@
 """Dataflow-hazard check of the step programs at BASELINE.json's full sizes, on the host simulation (no GPU):
 
-    python tools/hazard_check_configs.py [cfg2] [cfg3] [cfg4] [ais-depth]
+    python tools/hazard_check_configs.py [cfg2] [cfg3] [cfg4] [ais-depth] [ais-clamped]
 
 Every element a program launch reads or writes is shadowed while the launch is interpreted (tests/hostsim/kernels_cpu.cpp,
 `Hazards`); a read of / write over something another op of the launch touched must be covered by a declared dependency path,
@@ -8,7 +8,9 @@ Every element a program launch reads or writes is shadowed while the launch is i
 cfg3: Gaussian RBM 3072-5000, batch 512 (host batch and resident-dataset step).  cfg4: the tensor-core DBM engine's mean-field
 and particle programs, 784-512-1024, batch = particles = 1024.  ais-depth (not run by default): the AIS ladders of
 DbmTC::ais_local_layers at one, three and four hidden layers (100-64, 100-64-48-32, 100-64-48-32-16; 600 runs = three 256-run
-blocks, 40 temperatures, k = 2, several launches per ladder).  About 3 minutes, 2 GB."""
+blocks, 40 temperatures, k = 2, several launches per ladder).  ais-clamped (not run by default): the same ladders with v clamped
+(DESIGN.md §5.4g) at two, three and four hidden layers, 6 rows x 100 runs, on the host-simulation library that also restates
+the clamped ladder's operand kernel (build_dbm_ais_clamped.sh).  About 3 minutes, 2 GB."""
 import ctypes as C
 import os
 import subprocess
@@ -25,9 +27,11 @@ for p in (ROOT, os.path.join(ROOT, 'boltzmann-machines_b200')):
 
 def main():
     which = sys.argv[1:] or ['cfg2', 'cfg3', 'cfg4']
-    subprocess.check_call(['bash', os.path.join(ROOT, 'tests', 'hostsim', 'build.sh')], stdout=subprocess.DEVNULL)
+    name = 'dbm_ais_clamped' if 'ais-clamped' in which else ''
+    subprocess.check_call(['bash', os.path.join(ROOT, 'tests', 'hostsim', 'build_' + name + '.sh' if name else 'build.sh')],
+                          stdout=subprocess.DEVNULL)
     from boltzmann_machines import _native
-    sim = _native.load_library(os.path.join(ROOT, 'tests', 'hostsim', '_build', 'libbm_hostsim.so'))
+    sim = _native.load_library(os.path.join(ROOT, 'tests', 'hostsim', '_build', 'libbm_hostsim' + ('_' + name if name else '') + '.so'))
     sim.fakecuda_violation.restype = C.c_char_p
     sim.fakecuda_hazard_launches.restype = C.c_long
     sim.fakecuda_set_execute(1)
@@ -92,6 +96,22 @@ def main():
             eng.set_params(d)
             eng.ais(600, 40, 2, 3)
             ok = report('AIS ladder at {0} hidden layers'.format(L)) and ok
+            eng.close()
+    if 'ais-clamped' in which:
+        for Hs in ((64, 48), (64, 48, 32), (64, 48, 32, 16)):
+            V, L = 100, len(Hs)
+            cfg = dict(n_visible=V, n_hiddens=list(Hs), v_kind='bernoulli', h_kinds=['bernoulli'] * L, dtype='float32',
+                       compute='bf16', n_particles=16, batch_size=16, sample_v=True, sample_h=[True] * L)
+            eng = _native.CudaDBM(cfg)
+            sizes = [V] + list(Hs)
+            d = {'vb': np.zeros(V, np.float32)}
+            for i in range(L):
+                s = '' if i == 0 else '_%d' % i
+                d['W' + s] = (0.1 * rng.randn(sizes[i], sizes[i + 1])).astype(np.float32)
+                d['hb' + s] = np.zeros(sizes[i + 1], np.float32)
+            eng.set_params(d)
+            eng.ais_clamped((rng.rand(6, V) < 0.3).astype(np.float32), 100, 40, 2, 3)
+            ok = report('clamped AIS ladder at {0} hidden layers'.format(L)) and ok
             eng.close()
     sys.exit(0 if ok else 1)
 
